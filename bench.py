@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark: GPT-2-XL training tokens/s through the Oobleck pipeline-execution hot path.
 
-    python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_90a)
     python bench.py --impl reference --gpus N --steps K ...   # the reference path's CPU restatement (oracle port)
     python bench.py --gpus 8 --replicas 2 --model gpt2        # BASELINE config 4: 2 replicas x 4 stages (DP all-reduce)
     python bench.py --reconfig --gpus 8 --replicas 2          # second half of the metric: kill a rank, time the recovery
@@ -16,9 +16,12 @@ At N >= 4 the line also carries ``"reconfiguration"``: after the timed region ra
 the same GPUs (2 replicas x N/2 stages, and one N-stage pipeline with peer shadows), each SIGKILLing a worker inside a
 training step, and records the time from the lost-node message to the first completed step.  ``--with-reconfig 0`` /
 ``OOB_BENCH_RECONFIG=0`` turns it off; ``OOB_BENCH_RECONFIG_BUDGET_S`` (150) bounds each run, ``OOB_BENCH_EXTRAS_BUDGET_S``
-(400) all extras of a line together (the driver allows one bench.py run 870 s).  At N = 8 a third
+(400) all extras of a line together.  At N = 8 a third
 bounded extra follows, ``"config4_dp2_x_pp4"``: BASELINE config 4 itself (GPT-2 124M, 2 replicas x 4 stages) through this
 script in a torchrun of its own (``OOB_BENCH_CONFIG4=0`` skips it).
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed step computed (``LastStepCapture``) as .npy
+files: the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -66,8 +69,8 @@ def measured_peaks():
                     "hbm_gbs": float(d.get("hbm_gbs")), "source": "measured"}
         except Exception:  # noqa: BLE001
             pass
-    # /opt/skills/guides/B200_PROFILING.md fallback (sustained figure: the GEMMs are timed inside a long step)
-    return {"bf16_tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3), not a measured figure
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
 
 
 def workload_config(model: str, cfg: dict, gpus: int, replicas: int) -> dict:
@@ -102,7 +105,7 @@ def free_port() -> int:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -142,8 +145,7 @@ class ClockSampler:
 # micro-batch 1 x REF_SEQ tokens, P micro-batches per step.  Nothing is extrapolated: ``value`` is the tokens the sample
 # really processed divided by the wall time it really took (max over the processes).
 REF_SEQ = int(os.environ.get("OOB_REF_SEQ", "256"))
-# wall-clock budget of one CPU-arm run (the driver gives `bench.py --impl reference` 870 s; typical on a 16-core quota:
-# 7-9 s per step, 25 steps in about 220 s): past it the run stops after the current step and reports what it timed
+# wall-clock budget of one CPU-arm run: past it the run stops after the current step and reports what it timed
 CPU_ARM_BUDGET_S = float(os.environ.get("OOB_CPU_ARM_BUDGET_S", "600"))
 
 
@@ -335,7 +337,7 @@ def parity_check(args, cfg, world: int, rank: int, local_rank: int, transport_cl
     """Before anything is timed: the benchmarked configuration (width, heads, T, micro-batch, operand format, the same
     number of pipeline stages over the same transport) at reduced depth -- one train step of 2 micro-batches -- against
     the oracle on the host: total loss and the global L2 norm of all parameter gradients.  Raises if either is off, so a
-    line that was printed carries a passed check (and makes multi-GPU parity visible in the driver's records)."""
+    line that was printed carries a passed check."""
     import torch.distributed as dist
 
     from oobleck_b200.execution.dataloader import OobleckSampler, SyntheticTokenDataset
@@ -470,7 +472,7 @@ def run_ours(args, cfg):
             dist.barrier()
         torch.cuda.synchronize()
 
-    def timed(nsteps: int, device_resident: bool, read_loss: bool, time_gemms: bool = False):
+    def timed(nsteps: int, device_resident: bool, read_loss: bool, time_gemms: bool = False, capture=None):
         loader.device_resident = device_resident
         engine._pipeline.reset_iterator()
         barrier()
@@ -484,7 +486,11 @@ def run_ours(args, cfg):
                 L.call("oob_side_stream_enable", 0)
                 fb_saved, _pipeline.FB_OVERLAP = _pipeline.FB_OVERLAP, False
                 L.call("oob_gemm_timing_begin")
+            if capture is not None and i == nsteps - 1:
+                capture.arm()
             engine._train_step()
+            if capture is not None and i == nsteps - 1:
+                capture.disarm()
             if time_gemms and i == nsteps - 1:
                 L.call("oob_side_stream_enable", args.side_stream)
                 _pipeline.FB_OVERLAP = fb_saved
@@ -504,8 +510,11 @@ def run_ours(args, cfg):
     sampler = ClockSampler(local_rank)
     launches0 = L.load().oob_launch_count()
     sampler.start()
-    ms, _ = timed(args.steps, True, False, time_gemms=True)
+    capture = LastStepCapture(engine) if args.dump_outputs and rank < stages else None   # one replica: the others
+    ms, _ = timed(args.steps, True, False, time_gemms=True, capture=capture)            # hold the same layers
     clocks = sampler.stop()
+    if capture is not None:
+        capture.write(args.dump_outputs)
     launches = L.load().oob_launch_count() - launches0
     g_ms, g_fl, g_ex, g_n = C.c_double(), C.c_double(), C.c_double(), C.c_long()
     L.call("oob_gemm_timing_end", C.byref(g_ms), C.byref(g_fl), C.byref(g_ex), C.byref(g_n))
@@ -551,15 +560,15 @@ def run_ours(args, cfg):
         "metric": "training_tokens_per_s", "value": value, "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong",
         "vs_baseline": None,
-        "dtype": (("f32 (fp16 x2 planes forward and backward (loss-scaled) on tcgen05, fp32 accumulate + promotion)"
+        "dtype": (("f32 (fp16 x2 planes forward and backward (loss-scaled) on wgmma, fp32 accumulate + promotion)"
                    if bwd_fp16 else
-                   "f32 (fp16 x2 planes forward / bf16 x3 planes backward on tcgen05, fp32 accumulate + promotion)")
-                  if args.nsplit == 3 else "split-bf16 x%d on tcgen05, fp32 accumulate" % args.nsplit),
+                   "f32 (fp16 x2 planes forward / bf16 x3 planes backward on wgmma, fp32 accumulate + promotion)")
+                  if args.nsplit == 3 else "split-bf16 x%d on wgmma, fp32 accumulate" % args.nsplit),
         "data": "synthetic",
         "config": workload_config(args.model, cfg, world, args.replicas),
         "engine": {"nsplit": args.nsplit, "wgrad_side_stream": bool(args.side_stream), "bwd_fp16": bwd_fp16,
                    "fb_overlap": bool(_pipeline.FB_OVERLAP), "fb_overlap_multi_stage": bool(_pipeline.FB_OVERLAP_PP),
-                   "l2": "working set per step (>6 GB of weights) far exceeds the 126 MB L2; no flush needed",
+                   "l2": "working set per step (>6 GB of weights) far exceeds the 50 MB L2; no flush needed",
                    "stage_layers": [len(s._layer_indices) for s in template.get_stages()],
                    "stage_balance_from": engine.layer_costs_source,
                    "tensor_map_encodes": int(L.load().oob_tensor_map_encodes())},
@@ -573,10 +582,10 @@ def run_ours(args, cfg):
                 "d2h_bytes_per_step": 4 * args.replicas, "loss": last_loss},
         "model_flops_fraction_of_bf16_peak": value * fpt / (world * peaks["bf16_tflops"] * 1e12),
         "roofline": {
-            "bound": "tensor", "kernel": "gemm_bf16x3_persistent_kernel (tcgen05, all GEMM launches of the last timed step)",
+            "bound": "tensor", "kernel": "gemm_planes_sm90_kernel (wgmma, all GEMM launches of the last timed step)",
             "achieved": gemm_tflops, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
             "frac": (gemm_tflops / peaks["bf16_tflops"]) if gemm_tflops else None,
-            "peak_source": peaks["source"] + " (cuBLAS bf16, sustained)",
+            "peak_source": peaks["source"],
             "tensor_products_per_algorithmic_flop": (g_ex.value / g_fl.value) if g_fl.value else None,
             "products_note": "GEMMs on fp16 x 2 planes issue 3 products per MAC, on bf16 x 3 planes 6: with 3 products "
                              "the algorithmic ceiling is peak / 3; executed_frac_of_peak is the tensor-pipe reading",
@@ -585,8 +594,6 @@ def run_ours(args, cfg):
             "launches_timed": int(g_n.value),
             "timing_note": "the last timed step runs without the wgrad side stream and without forward/backward "
                            "stream overlap, so each GEMM launch is timed alone",
-            "traffic": GEMM_TRAFFIC_BYTES if args.model == "gpt2-xl" and args.nsplit == 3 and bwd_fp16 else None,
-            "traffic_note": GEMM_TRAFFIC_NOTE,
         },
     }
     if world == 1 and args.cpu_baseline:
@@ -622,8 +629,7 @@ def run_ours(args, cfg):
         dist.destroy_process_group()
 
 
-# The driver gives one bench.py run 870 s (SCALE_r01.json per_n_timeout_s).  The extras after the timed region are bounded
-# twice: each run by RECONFIG_BUDGET_S (typical: 40-60 s), all of them together by EXTRAS_BUDGET_S -- a run that would
+# The extras after the timed region are bounded twice: each run by RECONFIG_BUDGET_S (typical: 40-60 s), all of them together by EXTRAS_BUDGET_S -- a run that would
 # start with less than 45 s left is skipped and says so -- so the throughput line is printed in time whatever happens.
 RECONFIG_BUDGET_S = float(os.environ.get("OOB_BENCH_RECONFIG_BUDGET_S", "150"))
 EXTRAS_BUDGET_S = float(os.environ.get("OOB_BENCH_EXTRAS_BUDGET_S", "400"))
@@ -734,14 +740,69 @@ def embedded_reconfiguration(model: str, world: int, deadline: float | None = No
     return out
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant GEMM shape in the DEFAULT build (fp16 pairs
-# everywhere, pair-only plane buffers): forward FC 2048 x 6400 x 1600, bias + GELU epilogue writing the fp32
-# pre-activation and the two fp16 planes of GELU(x).  Source: profiles/ (see GEMM_TRAFFIC_NOTE).
-GEMM_TRAFFIC_BYTES = 54.50e6 + 57.77e6
-GEMM_TRAFFIC_NOTE = ("bytes/launch (dram read 54.5 MB + write 57.8 MB) from ncu --set full of the forward-FC launch in the "
-                     "default pair-only build, profiles/r02_ncu_gemm_fwdfc_pair_2groups.txt; algorithmic bytes of that "
-                     "launch: 54 MB of operand planes + 105 MB of outputs (part of the output is still in L2 when the "
-                     "kernel ends); `achieved` aggregates all GEMM shapes")
+# --dump-outputs: per layer at most DUMP_SAMPLE elements of the gradients and of the parameters (a fixed, seeded sample
+# of the larger ones) -- 50 GPT-2-XL stage layers x 2 x 128 Ki float32 = 50 MB, under the 64 MB the dump may take
+DUMP_SAMPLE = 1 << 17
+
+
+def _dump_sample(t: torch.Tensor, layer_id: int) -> torch.Tensor:
+    """The whole vector, or the same seeded sample of DUMP_SAMPLE of its elements on every run (a device copy)."""
+    v = t.detach().reshape(-1)
+    if v.numel() > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(1000 + layer_id)
+        idx = torch.randint(0, v.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+        return v[idx.to(v.device)]
+    return v.clone()
+
+
+class LastStepCapture:
+    """What one train step hands its caller, captured inside that step: its loss, the gradients it accumulated (taken
+    right before ``optimizer_step``, which applies and then zeroes them) and the parameters after the update.
+
+    ``arm()`` before the step: the execution's running ``total_loss`` (a sum over every step so far) is swapped for a
+    zero tensor so that the step's own loss accumulates alone, and ``optimizer_step`` is wrapped to copy the gradients
+    first.  ``disarm()`` after it restores both (the running sum continues with the step's loss added).  Capturing
+    costs the timed step one device synchronisation and a gather per layer."""
+
+    def __init__(self, engine):
+        self.engine = engine
+        self.loss = None
+        self.grads = {}
+        self.params = {}
+
+    def arm(self):
+        ex = self.engine._pipeline.execution
+        self._running = ex.total_loss
+        if self._running is not None:
+            ex.total_loss = torch.zeros_like(self._running)
+        inner = ex.optimizer_step
+
+        def optimizer_step(*a, **kw):
+            torch.cuda.synchronize()      # every stream's gradient work of the step is done
+            self.grads = {l.layer_id: _dump_sample(l.flat_grad, l.layer_id) for l in ex._layers if l.flat_grad is not None}
+            return inner(*a, **kw)
+        ex.optimizer_step = optimizer_step
+
+    def disarm(self):
+        ex = self.engine._pipeline.execution
+        del ex.optimizer_step             # back to the class's method
+        if ex.total_loss is not None:     # last stage
+            self.loss = ex.total_loss.clone()
+            if self._running is not None:
+                ex.total_loss = self._running + ex.total_loss
+        self.params = {l.layer_id: _dump_sample(l.flat_param, l.layer_id) for l in ex._layers}
+
+    def write(self, out_dir: str) -> None:
+        """``loss.npy`` (float64, last stage only), per stage layer ``layer<ID>_grad.npy`` and ``layer<ID>_param.npy``
+        (float32) in ``out_dir``."""
+        import numpy as np
+        os.makedirs(out_dir, exist_ok=True)
+        torch.cuda.synchronize()
+        if self.loss is not None:
+            np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(self.loss.double().item())], dtype=np.float64))
+        for name, d in (("grad", self.grads), ("param", self.params)):
+            for layer_id, v in d.items():
+                np.save(os.path.join(out_dir, f"layer{layer_id:03d}_{name}.npy"), v.float().cpu().numpy())
 
 
 def main():
@@ -767,6 +828,10 @@ def main():
     ap.add_argument("--with-reconfig", type=int, default=int(os.environ.get("OOB_BENCH_RECONFIG", "1")), choices=[0, 1],
                     help="N >= 4: after the timed region, also kill a rank of a fresh job on the same GPUs and report "
                          "the recovery time under \"reconfiguration\" (adds 2-3 minutes)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last timed step's loss, gradients (before the optimizer "
+                         "step) and updated parameters (seeded samples of the large ones) to DIR as .npy files; "
+                         "bench_outputs/ is git-ignored")
     ap.add_argument("--reconfig", action="store_true",
                     help="reconfiguration latency after a real kill of one rank (spawns its own workers; see "
                          "tools/reconfig_bench.py)")

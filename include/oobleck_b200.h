@@ -1,4 +1,4 @@
-/* oobleck_b200 -- C ABI of the B200-native kernel library behind Oobleck's pipeline-execution hot path.
+/* oobleck_b200 -- C ABI of the H100-native (sm_90a) kernel library behind Oobleck's pipeline-execution hot path.
  *
  * The reference (SymbioticLab/Oobleck @ 3b7a0c2f) has NO native boundary on this path: every stage layer is a
  * torch.fx.GraphModule of HF GPT-2 modules run by torch eager (oobleck/execution/layer.py:144-145,
@@ -10,7 +10,7 @@
  *   - every function returns 0 on success, <0 on error; oob_last_error() returns the message (thread local)
  *   - all data pointers are CUDA device pointers owned by the caller (torch tensors' data_ptr()); `stream` is a
  *     cudaStream_t passed as void*; nothing synchronises the device or allocates device memory
- *   - "planes" are the split 16-bit representation of an fp32 matrix, what the tcgen05 GEMMs consume
+ *   - "planes" are the split 16-bit representation of an fp32 matrix, what the wgmma GEMMs consume
  *     (DESIGN.md "Numerics"): [nplanes][rows][ld] 2-byte elements.  Planes 0-2 are bf16 with x == p0 + p1 + p2 to
  *     24 bits (any range: gradients, everything in backward).  A 5-plane buffer additionally carries, as planes 3-4,
  *     the fp16 pair x ~= h0 + 2^-11 h1 (22 bits, bounded range: weights and forward activations), which needs half
@@ -29,7 +29,7 @@ extern "C" {
 int oob_version(void);
 const char* oob_last_error(void);
 /* instrumentation used by bench.py: kernels launched so far by this library, and CUDA-event timing of every
- * tcgen05 GEMM launch between begin/end (events are recorded on the launching stream; end synchronises them) */
+ * GEMM launch between begin/end (events are recorded on the launching stream; end synchronises them) */
 long oob_launch_count(void);
 /* host-side cuTensorMapEncodeTiled calls so far (TMA descriptors are cached per (buffer, shape, box)) */
 long oob_tensor_map_encodes(void);
@@ -124,7 +124,7 @@ int oob_adamw_step(float* param, const float* grad, float* exp_avg, float* exp_a
  * ``for layer in self._layers: inputs = layer(inputs)`` (pipeline.py:188-189) and Layer.backward's
  * torch.autograd.backward (layer.py:250-260) turn into.  The reference re-computes block forwards under
  * checkpoint_wrapper (layer.py:93-94); here forward saves what backward needs into a caller-owned oob_block_ctx
- * (one per in-flight micro-batch, 180 GB of HBM makes recomputation unnecessary). */
+ * (one per in-flight micro-batch; 80 GB of HBM hold them at the benchmarked sizes, so nothing is recomputed). */
 typedef struct oob_dims {
   int batch, seq;          /* micro-batch shape: M = batch*seq rows */
   int n_embd, n_head;      /* head_dim = n_embd / n_head must be 64 */

@@ -1,5 +1,5 @@
-// Shared device/host helpers for the sm_100a kernels: error plumbing, inline-PTX wrappers for
-// mbarrier / TMA / tcgen05 / TMEM, and the split-bf16 ("bf16x3") representation of fp32 operands.
+// Shared device/host helpers for the sm_90a kernels: error plumbing, inline-PTX wrappers for
+// mbarrier / TMA / wgmma, and the split-bf16 ("bf16x3") representation of fp32 operands.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -115,7 +115,7 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// PTX wrappers (sm_100a)
+// PTX wrappers (sm_90a)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
@@ -167,78 +167,48 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// TMEM allocation: whole warp, writes base address to *smem_slot.  ncols power of two >= 32.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate.  One thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// tcgen05.commit: arrive on an mbarrier when all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive 32-bit columns; thread i of the warp gets lane (base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor (tcgen05), see PTX ISA "Matrix Descriptor" / cute::UMMA::SmemDescriptor:
-//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [46,48) version=1  [49,52) base offset  [61,64) swizzle
-enum : uint64_t { SWZ_NONE = 0, SWZ_128B = 2, SWZ_64B = 4, SWZ_32B = 6 };
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint64_t swizzle) {
+// Shared-memory matrix descriptor (wgmma), PTX ISA "Matrix Descriptor Format" / cute::GMMA::GmmaDescriptor:
+//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [49,52) base offset  [62,64) layout (1 = 128-B swizzle)
+// Every tile here is a stack of 128-B rows in the SWIZZLE_128B pattern TMA writes, 1024-B aligned:
+//  K-major  : SBO = 1024 (8-row groups); a k-step of 16 elements advances the start address by 32 B
+//  MN-major : LBO = distance between 64-element MN atoms, SBO = 1024; a k-step of 16 rows advances it by 2048 B
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= swizzle << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16 with fp32 accumulation (cute::UMMA::InstrDescriptor); operand formats:
-// 1 = BF16, 0 = F16 (independent fields for A and B)
-__host__ __device__ constexpr uint32_t make_idesc_f16kind(int M, int N, int a_mn_major, int b_mn_major,
-                                                          int a_bf16 = 1, int b_bf16 = 1) {
-  return (1u << 4)                       // c_format  = F32
-         | ((uint32_t)a_bf16 << 7)       // a_format
-         | ((uint32_t)b_bf16 << 10)      // b_format
-         | ((uint32_t)a_mn_major << 15)  // a_major   (0 = K-major, 1 = MN-major)
-         | ((uint32_t)b_mn_major << 16)  // b_major
-         | ((uint32_t)(N >> 3) << 17)    // n_dim
-         | ((uint32_t)(M >> 4) << 24);   // m_dim
+
+// warpgroup MMA (sm_90a): D[64 x N] (fp32 registers) (+)= A[64 x 16] . B[16 x N], both operands from shared memory.
+// TA / TB: 0 = K-major, 1 = MN-major.  The four instruction variants are in wgmma_sm90.inc.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma_wait
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+#include "wgmma_sm90.inc"
+template <bool F16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (F16) wgmma_m64n128_f16<TA, TB>(d, a, b, scale_d);
+  else wgmma_m64n128_bf16<TA, TB>(d, a, b, scale_d);
+}
+template <bool F16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (F16) wgmma_m64n64_f16<TA, TB>(d, a, b, scale_d);
+  else wgmma_m64n64_bf16<TA, TB>(d, a, b, scale_d);
+}
+// Accumulator fragment of an m64nN wgmma: register i of thread (warp w of the warpgroup, lane l) holds
+// row 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1).
+__device__ __forceinline__ int frag_row(int warp_in_wg, int lane, int i) { return 16 * warp_in_wg + (lane >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int lane, int i) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 // 128-bit streaming global accesses

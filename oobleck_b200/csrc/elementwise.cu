@@ -1,4 +1,4 @@
-// HBM-bound kernels of the stage layers (sm_100a): split, LayerNorm fwd/bwd, column reductions (bias grads),
+// HBM-bound kernels of the stage layers (sm_90a): split, LayerNorm fwd/bwd, column reductions (bias grads),
 // embedding gather / scatter, shifted cross-entropy, fused AdamW.  All are warp-shuffle kernels with 128-bit
 // coalesced accesses; none stages through shared memory except for the cross-warp reductions.
 #include "kernels.h"
@@ -49,7 +49,7 @@ int split_planes(const float* x, bf16* planes, long n, long plane_stride, int np
             "split_planes: misaligned buffers");
   if (n <= 0) return 0;
   int blocks = (int)((n / 4 + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   split_kernel<<<blocks, 256, 0, s>>>(x, planes, n, plane_stride, nplanes);
   OOB_CUDA_OK(cudaGetLastError());
@@ -586,7 +586,7 @@ int adamw_step(float* p, const float* g, float* m, float* v, bf16* planes, long 
   const double bc1 = 1.0 - pow((double)beta1, step);
   const double bc2 = 1.0 - pow((double)beta2, step);
   long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   adamw_kernel<<<(int)blocks, 256, 0, s>>>(p, g, m, v, planes, plane_stride, nplanes, n, lr, beta1, beta2, eps, wd,
                                            (float)bc1, (float)sqrt(bc2));

@@ -1,13 +1,11 @@
-// Host launcher for the tcgen05 split-plane GEMM: builds the TMA tensor maps and picks the stage count.
+// Host launcher for the wgmma split-plane GEMM: builds the TMA tensor maps and picks the stage count.
 #include <atomic>
 #include <cstdlib>
 #include <mutex>
 #include <unordered_map>
 #include <vector>
 
-#include "gemm_sm100.cuh"
-#include "gemm_sm100_2cta.cuh"
-#include "gemm_sm100_persistent.cuh"
+#include "gemm_sm90.cuh"
 
 namespace oob {
 
@@ -28,9 +26,9 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 3-D map over [planes][rows][ld] bf16; box = {bk elements, box_rows, box_planes}; bk = 64 -> SWIZZLE_128B,
-// bk = 32 -> SWIZZLE_64B (one smem row is exactly one swizzle span, see KCfg).
-static int make_map(CUtensorMap* m, const PlaneMat& a, int box_rows, int box_planes, int bk) {
+// 3-D map over [planes][rows][ld] bf16; box = {64 elements, box_rows, box_planes}, SWIZZLE_128B (one smem row is
+// exactly one swizzle span).
+static int make_map(CUtensorMap* m, const PlaneMat& a, int box_rows, int box_planes) {
   EncodeTiledFn enc = get_encode_fn();
   OOB_CHECK(enc != nullptr, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   OOB_CHECK((a.ld % 8) == 0 && (a.plane_stride % 8) == 0, "split-plane operand strides must be multiples of 8");
@@ -38,10 +36,10 @@ static int make_map(CUtensorMap* m, const PlaneMat& a, int box_rows, int box_pla
   OOB_CHECK(box_planes <= a.nplanes, "GEMM asks for %d planes, operand has %d", box_planes, a.nplanes);
   cuuint64_t dims[3] = {(cuuint64_t)a.cols, (cuuint64_t)a.rows, (cuuint64_t)a.nplanes};
   cuuint64_t strides[2] = {(cuuint64_t)a.ld * 2, (cuuint64_t)a.plane_stride * 2};
-  cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)box_rows, (cuuint32_t)box_planes};
+  cuuint32_t box[3] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows, (cuuint32_t)box_planes};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(a.base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   OOB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d): rows=%ld cols=%ld ld=%ld", (int)r, a.rows, a.cols,
@@ -50,14 +48,14 @@ static int make_map(CUtensorMap* m, const PlaneMat& a, int box_rows, int box_pla
 }
 
 // Descriptor cache.  A training step launches the same few hundred (buffer, shape, box) combinations every micro-batch
-// (round 1 encoded two maps per GEMM on the host: 74 k cuTensorMapEncodeTiled calls per GPT-2-XL step); a map depends
+// (encoding two maps per GEMM on the host costs tens of thousands of cuTensorMapEncodeTiled calls per GPT-2-XL step); a map depends
 // only on the key below, never on the buffer's contents, so entries stay valid for as long as the address is reused
 // for the same shape.  Per host thread (no lock); bounded.
 struct MapKey {
-  const void* base; long rows, cols, ld, plane_stride; int nplanes, box_rows, box_planes, bk;
+  const void* base; long rows, cols, ld, plane_stride; int nplanes, box_rows, box_planes;
   bool operator==(const MapKey& o) const {
     return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && plane_stride == o.plane_stride &&
-           nplanes == o.nplanes && box_rows == o.box_rows && box_planes == o.box_planes && bk == o.bk;
+           nplanes == o.nplanes && box_rows == o.box_rows && box_planes == o.box_planes;
   }
 };
 struct MapKeyHash {
@@ -65,21 +63,21 @@ struct MapKeyHash {
     size_t h = reinterpret_cast<size_t>(k.base) * 0x9E3779B97F4A7C15ull;
     auto mix = [&h](size_t v) { h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2); };
     mix((size_t)k.rows); mix((size_t)k.cols); mix((size_t)k.ld); mix((size_t)k.plane_stride);
-    mix((size_t)k.nplanes * 1000003u + (size_t)k.box_rows * 10007u + (size_t)k.box_planes * 101u + (size_t)k.bk);
+    mix((size_t)k.nplanes * 1000003u + (size_t)k.box_rows * 10007u + (size_t)k.box_planes * 101u);
     return h;
   }
 };
 static std::atomic<long> g_map_encodes{0};
 long tensor_map_encodes() { return g_map_encodes.load(); }
 
-int tensor_map_3d(const CUtensorMap** out, const PlaneMat& a, int box_rows, int box_planes, int bk) {
+int tensor_map_3d(const CUtensorMap** out, const PlaneMat& a, int box_rows, int box_planes) {
   thread_local std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-  const MapKey key{a.base, a.rows, a.cols, a.ld, a.plane_stride, a.nplanes, box_rows, box_planes, bk};
+  const MapKey key{a.base, a.rows, a.cols, a.ld, a.plane_stride, a.nplanes, box_rows, box_planes};
   auto it = cache.find(key);
   if (it == cache.end()) {
     if (cache.size() >= 16384) cache.clear();
     CUtensorMap m;
-    if (int rc = make_map(&m, a, box_rows, box_planes, bk)) return rc;
+    if (int rc = make_map(&m, a, box_rows, box_planes)) return rc;
     g_map_encodes.fetch_add(1, std::memory_order_relaxed);
     it = cache.emplace(key, m).first;
   }
@@ -115,55 +113,34 @@ int gemm_timing_end(double* total_ms, double* total_flops, double* executed_flop
   return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, bool TWO_CTA, int BK>
-static int launchp_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, cudaStream_t stream) {
-  static int max_smem = -1, num_sms = 0;
+template <bool A_MN, bool B_MN, bool F16>
+static int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+  static int max_smem = -1;
   if (max_smem < 0) {
     int dev = 0;
     OOB_CUDA_OK(cudaGetDevice(&dev));
     OOB_CUDA_OK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    OOB_CUDA_OK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
   }
   static bool attr_set = false;
-  auto kern = gemm_bf16x3_persistent_kernel<BN, A_MN, B_MN, TWO_CTA, BK>;
+  auto kern = gemm_planes_sm90_kernel<A_MN, B_MN, F16>;
   if (!attr_set) {
     OOB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     attr_set = true;
   }
-  GemmParams p = p_in;
-  const int stage = gemmp_stage_bytes<BN, TWO_CTA, BK>(p.nsplit);
-  // epilogue transposition tiles: one per epilogue warp, 32 rows x slab fp32; 32-column slabs (full 128-B lines per
-  // store) unless they would cost a ring stage
-  constexpr int EPI_WARPS = 4 * GEMM_EPI_GROUPS;
-  int overhead = 1024 + 256 + EPI_WARPS * 32 * 32 * 4;
-  p.slab = 32;
-  if ((max_smem - overhead) / stage < (max_smem - (overhead - EPI_WARPS * 32 * 16 * 4)) / stage) {
-    overhead -= EPI_WARPS * 32 * 16 * 4;
-    p.slab = 16;
-  }
+  const int stage = gemm_stage_bytes(p.nsplit);
+  const int overhead = 1024 + 256;   // alignment slack, barriers
   int stages = (max_smem - overhead) / stage;
-  if (stages > 10) stages = 10;
-  OOB_CHECK(stages >= 2, "persistent GEMM tile does not fit %d B of shared memory", max_smem);
-  const int tile_m = TWO_CTA ? 2 * GEMM_BM : GEMM_BM;
-  const int tiles = ((p.M + tile_m - 1) / tile_m) * ((p.N + BN - 1) / BN);
-  const int max_units = TWO_CTA ? num_sms / 2 : num_sms;
-  const int units = tiles < max_units ? tiles : max_units;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(TWO_CTA ? 2 * units : units);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = (size_t)stages * stage + overhead;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = TWO_CTA ? 2 : 1;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  if (stages > 8) stages = 8;
+  OOB_CHECK(stages >= 2, "GEMM tile does not fit %d B of shared memory", max_smem);
+  OOB_CHECK((size_t)stages * stage >= sizeof(float) * GEMM_BM * GEMM_STAGE_LD, "GEMM epilogue staging does not fit");
+  const dim3 grid((p.M + GEMM_BM - 1) / GEMM_BM, (p.N + GEMM_BN - 1) / GEMM_BN);
+  OOB_CHECK(grid.y <= 65535, "GEMM N = %d too large", p.N);
+  const size_t smem = (size_t)stages * stage + overhead;
   TimedLaunch tl{};
   if (g_timing) { tl.a = get_event(); tl.b = get_event(); tl.flops = 2.0 * p.M * p.N * p.K;
     tl.executed = tl.flops * (p.nsplit == 1 ? 1 : (p.nsplit == 2 ? 3 : 6)); cudaEventRecord(tl.a, stream); }
-  OOB_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ta, tb, p, stages));
+  kern<<<grid, GEMM_THREADS, smem, stream>>>(ta, tb, p, stages);
+  OOB_CUDA_OK(cudaGetLastError());
   if (g_timing) { cudaEventRecord(tl.b, stream); g_timed.push_back(tl); }
   count_launch();
   return 0;
@@ -171,72 +148,55 @@ static int launchp_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPar
 
 int gemm_launch(const PlaneMat& A, int a_mn, const PlaneMat& B, int b_mn, const GemmParams& p_in, cudaStream_t stream) {
   GemmParams p = p_in;
-  static const int env_chunk = [] { const char* e = getenv("OOB_GEMM_CHUNK_KB"); return e ? atoi(e) : 0; }();
-  if (p.chunk_kb <= 0) p.chunk_kb = env_chunk;
-  static const int env_debug = [] { const char* e = getenv("OOB_GEMM_DEBUG"); return e ? atoi(e) : 0; }();
-  p.debug = env_debug;
   OOB_CHECK(p.nsplit >= 1 && p.nsplit <= 3, "nsplit must be 1..3");
   OOB_CHECK(p.M > 0 && p.N > 0 && p.K > 0, "empty GEMM %d x %d x %d", p.M, p.N, p.K);
-  // operand formats: bf16 x (1..3) planes, or fp16 x (1..2) planes with the second plane pre-scaled by 2^11.  A and B
-  // formats are independent fields of the instruction descriptor, but the two correction products of a mixed pair
-  // would need different weights, so mixed operands are single-plane only.
-  p.a_bf16 = A.fp16 ? 0 : 1;
-  p.b_bf16 = B.fp16 ? 0 : 1;
+  // operand formats: bf16 x (1..3) planes, or fp16 x (1..2) planes with the second plane pre-scaled by 2^11.  wgmma
+  // takes one element type for both operands, so the two must agree.
+  OOB_CHECK(A.fp16 == B.fp16, "mixed fp16 / bf16 operands are not supported");
   p.corr_scale = 1.0f;
-  if (A.fp16 || B.fp16) {
+  if (A.fp16) {
     OOB_CHECK(p.nsplit <= 2, "fp16 planes come in pairs: nsplit must be 1 or 2");
-    OOB_CHECK(A.fp16 == B.fp16 || p.nsplit == 1, "mixed fp16 / bf16 operands are supported for nsplit = 1 only");
     if (p.nsplit == 2) p.corr_scale = 1.0f / 2048.0f;
   }
   OOB_CHECK(A.nplanes >= p.nsplit && B.nplanes >= p.nsplit, "operands carry fewer planes than nsplit");
   {
     GemmEpilogue& e = p.epi;
     auto ok16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-    static const int env_pf = [] { const char* v = getenv("OOB_EPI_PREFETCH"); return v ? atoi(v) : 1; }();
-    e.prefetch = env_pf;
     e.vec4 = (!e.d || (ok16(e.d) && (e.ldd & 3) == 0)) && (!e.bias || ok16(e.bias)) &&
              (!e.resid || (ok16(e.resid) && (e.ldr & 3) == 0)) && (!e.aux || (ok16(e.aux) && (e.ldaux & 3) == 0)) &&
              (!e.planes || ((reinterpret_cast<uintptr_t>(e.planes) & 7) == 0 && (e.ldp & 3) == 0 &&
                             (e.plane_stride & 3) == 0));
   }
-  constexpr int BN = 128;
-  // kernel selection (measured on B200, profiles/r01_gemm_sweep*.log): persistent 2-CTA pair tiles with BK = 64 win on
-  // every GPT-2 shape (1-CTA: -15 %, BK = 32 / SWIZZLE_64B: -12 %).  Env vars select the variants for experiments.
-  static const int env_2cta = [] { const char* e = getenv("OOB_GEMM_2CTA"); return e ? atoi(e) : -1; }();
-  static const int env_bk = [] { const char* e = getenv("OOB_GEMM_BK"); return e ? atoi(e) : -1; }();
-  const int use_2cta = env_2cta >= 0 ? env_2cta : 1;
-  const int bk = (env_bk == 32 || env_bk == 64) ? env_bk : 64;
   const CUtensorMap *pta = nullptr, *ptb = nullptr;
   int rc;
-  // K-major operand: stored [MN][K] -> box {bk k, tile rows, planes}; MN-major: stored [K][MN] -> box {bk mn, bk rows}
+  // K-major operand: stored [MN][K] -> box {64 k, tile rows, planes}; MN-major: stored [K][MN] -> box {64 mn, 64 k rows}
   if (!a_mn) {
     OOB_CHECK(A.rows >= p.M && A.cols >= p.K, "A (K-major) is %ld x %ld, need %d x %d", A.rows, A.cols, p.M, p.K);
-    rc = tensor_map_3d(&pta, PlaneMat{A.base, (long)p.M, (long)p.K, A.ld, A.plane_stride, A.nplanes}, GEMM_BM, p.nsplit, bk);
+    rc = tensor_map_3d(&pta, PlaneMat{A.base, (long)p.M, (long)p.K, A.ld, A.plane_stride, A.nplanes}, GEMM_BM, p.nsplit);
   } else {
     OOB_CHECK(A.rows >= p.K && A.cols >= p.M, "A (M-major) is %ld x %ld, need %d x %d", A.rows, A.cols, p.K, p.M);
-    rc = tensor_map_3d(&pta, PlaneMat{A.base, (long)p.K, (long)p.M, A.ld, A.plane_stride, A.nplanes}, bk, p.nsplit, bk);
+    rc = tensor_map_3d(&pta, PlaneMat{A.base, (long)p.K, (long)p.M, A.ld, A.plane_stride, A.nplanes}, GEMM_BK, p.nsplit);
   }
   if (rc) return rc;
   if (!b_mn) {
     OOB_CHECK(B.rows >= p.N && B.cols >= p.K, "B (K-major) is %ld x %ld, need %d x %d", B.rows, B.cols, p.N, p.K);
-    rc = tensor_map_3d(&ptb, PlaneMat{B.base, (long)p.N, (long)p.K, B.ld, B.plane_stride, B.nplanes}, use_2cta ? BN / 2 : BN,
-                  p.nsplit, bk);
+    rc = tensor_map_3d(&ptb, PlaneMat{B.base, (long)p.N, (long)p.K, B.ld, B.plane_stride, B.nplanes}, GEMM_BN, p.nsplit);
   } else {
     OOB_CHECK(B.rows >= p.K && B.cols >= p.N, "B (N-major) is %ld x %ld, need %d x %d", B.rows, B.cols, p.K, p.N);
-    rc = tensor_map_3d(&ptb, PlaneMat{B.base, (long)p.K, (long)p.N, B.ld, B.plane_stride, B.nplanes}, bk, p.nsplit, bk);
+    rc = tensor_map_3d(&ptb, PlaneMat{B.base, (long)p.K, (long)p.N, B.ld, B.plane_stride, B.nplanes}, GEMM_BK, p.nsplit);
   }
   if (rc) return rc;
   const CUtensorMap& ta = *pta;
   const CUtensorMap& tb = *ptb;
-#define OOB_DISPATCH_MAJORS(FN, ...)                                                       \
-  do {                                                                                      \
-    if (!a_mn && !b_mn) return FN<BN, false, false, __VA_ARGS__>(ta, tb, p, stream);        \
-    if (!a_mn && b_mn) return FN<BN, false, true, __VA_ARGS__>(ta, tb, p, stream);          \
-    if (a_mn && !b_mn) return FN<BN, true, false, __VA_ARGS__>(ta, tb, p, stream);          \
-    return FN<BN, true, true, __VA_ARGS__>(ta, tb, p, stream);                              \
+#define OOB_DISPATCH_MAJORS(F16)                                                  \
+  do {                                                                            \
+    if (!a_mn && !b_mn) return launch_t<false, false, F16>(ta, tb, p, stream);    \
+    if (!a_mn && b_mn) return launch_t<false, true, F16>(ta, tb, p, stream);      \
+    if (a_mn && !b_mn) return launch_t<true, false, F16>(ta, tb, p, stream);      \
+    return launch_t<true, true, F16>(ta, tb, p, stream);                          \
   } while (0)
-  if (use_2cta) { if (bk == 64) OOB_DISPATCH_MAJORS(launchp_t, true, 64); else OOB_DISPATCH_MAJORS(launchp_t, true, 32); }
-  if (bk == 64) OOB_DISPATCH_MAJORS(launchp_t, false, 64); else OOB_DISPATCH_MAJORS(launchp_t, false, 32);
+  if (A.fp16) OOB_DISPATCH_MAJORS(true);
+  OOB_DISPATCH_MAJORS(false);
 #undef OOB_DISPATCH_MAJORS
 }
 

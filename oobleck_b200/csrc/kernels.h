@@ -1,11 +1,11 @@
 // Internal C++ interface of the kernel library (one translation unit per kernel family).
 #pragma once
 #include "common.cuh"
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 
 namespace oob {
 
-constexpr int LN_BWD_MAX_GRID = 592;   // 4 CTAs per SM
+constexpr int LN_BWD_MAX_GRID = 528;   // 4 CTAs per SM (132 SMs)
 constexpr int COLSUM_MAX_PARTS = 64;
 
 int split_planes(const float* x, bf16* planes, long n, long plane_stride, int nplanes, cudaStream_t s);

@@ -1,16 +1,16 @@
-"""``Layer``: one stage layer materialised on a B200.
+"""``Layer``: one stage layer materialised on a GPU.
 
 Replaces oobleck/execution/layer.py:40-291.  The reference wraps a deep-copied fx GraphModule in an FSDP
 ``FlatParamHandle`` and lets torch.autograd run it; here a layer is
 
 * one flat fp32 parameter vector in HF ``parameters()`` order (``_param_handle.flat_param`` keeps the reference's
   attribute path so the reconfiguration / DP code that pokes it keeps working, engine.py:284-306),
-* its flat fp32 gradient (``flat_param.grad``), AdamW moments and the split-bf16 planes the tcgen05 GEMMs read,
+* its flat fp32 gradient (``flat_param.grad``), AdamW moments and the split-bf16 planes the wgmma GEMMs read,
 * per pipe-buffer activation contexts that the hand-written forward fills and the hand-written backward consumes
   (no autograd graph, no checkpoint recompute -- layer.py:93-94 re-runs every block forward in backward).
 
 A stage that owns several GPUs shards this state across them (layer.py:96-142, 167-225 -- FSDP ``FULL_SHARD``): see
-``sharding.py`` for the B200 schedule of it (one in-place all-gather and one reduce-scatter per layer and STEP).  Every
+``sharding.py`` for the GPU schedule of it (one in-place all-gather and one reduce-scatter per layer and STEP).  Every
 BASELINE config runs one GPU per stage, the reference's ``NO_SHARD`` branch (layer.py:100-102), which allocates exactly
 what it did before sharding existed.
 """

@@ -1,4 +1,4 @@
-"""Pipeline-parallel execution of one Oobleck pipeline on B200s.
+"""Pipeline-parallel execution of one Oobleck pipeline on H100s.
 
 Drop-in for oobleck/execution/pipeline.py: same class names, constructor signatures and attributes that the
 planner (``HeterogeneousPipelinesExecutionPlan.instantiate``, planning/instantiator.py:135-152), the engine
@@ -10,7 +10,7 @@ planner (``HeterogeneousPipelinesExecutionPlan.instantiate``, planning/instantia
     OobleckPipeline           rank grid, wiring, ``train()``        (pipeline.py:430-623)
 
 What changed underneath:
-* stage layers are ``oobleck_b200.execution.layer.Layer`` objects driving hand-written sm_100a kernels, with
+* stage layers are ``oobleck_b200.execution.layer.Layer`` objects driving hand-written sm_90a kernels, with
   hand-written backward (no autograd graph, no activation recomputation);
 * no ``dist.new_group`` per layer / per shard column: membership is plain arithmetic (``RankGroup``), so building or
   re-building a pipeline costs no collective (SURVEY 7 hard part 6);

@@ -7,9 +7,9 @@ gradient after every micro-batch backward into ``_saved_grad_shard`` (:167-225) 
 shard.  Cross-replica all-reduce then runs per ``fsdp_index`` on the shards (:272-291), a layer that is NOT sharded in one
 pipeline splitting its gradient with ``_shard_param`` (:262-270) to meet the shards of a pipeline where it is.
 
-Same state ownership here, scheduled for a B200:
+Same state ownership here, scheduled for the GPU:
 
-* parameters change once per step, and 180 GB of HBM hold every gathered layer of a stage: the all-gather runs ONCE per
+* parameters change once per step, and HBM holds every gathered layer of a stage: the all-gather runs ONCE per
   step (lazily, before the first forward after ``optimizer_step``), in place -- the local shard is a view into the
   gathered buffer, so neither the gather nor the optimizer copies anything.  ``reshard_params`` therefore has nothing to
   free (2 x micro_batches all-gathers per layer and step in the reference, 1 here);

@@ -174,7 +174,7 @@ class OobleckModel:
         torch.default_generator.manual_seed(RANDOM_SEED)
         if not any(key in model_name for key in lang_models):
             raise NotImplementedError(
-                f"{model_name}: only GPT-2-type models are on the B200 hot path (north_star); "
+                f"{model_name}: only GPT-2-type models are on the CUDA hot path (north_star); "
                 "bert/t5/vit/resnet split points (sharding.py:19-43) are out of scope")
         config_args = dict(config_args or {})
         config_args["use_cache"] = False                 # model.py:61-64

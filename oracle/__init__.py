@@ -5,7 +5,7 @@ package; only ``tests/``, ``__graft_entry__.smoke()`` and the ``cpu_baseline`` /
 ``--impl reference`` legs of ``bench.py`` do, and only as the checker / the
 reported CPU baseline -- never as the thing shipped.
 
-What it restates (reference = /root/reference @ 3b7a0c2f, never copied):
+What it restates (reference = SymbioticLab/Oobleck @ 3b7a0c2f, never copied):
 
 * ``schedule.py``     -- oobleck/execution/pipeline.py:24-84 (``OobleckPipelineSchedule.steps``)
                          on top of deepspeed ``TrainSchedule`` index math (third party,
@@ -23,14 +23,14 @@ What it restates (reference = /root/reference @ 3b7a0c2f, never copied):
 
 * ``_ref/``          -- not a restatement: the REFERENCE's own C++ planner module (``pipeline_template``,
                          oobleck/csrc/planning/{pipeline_template.cpp,bind.cpp}) built by ``make -C oracle``
-                         from the sources where they lie under /root/reference, with single-threaded
+                         from the sources of a reference checkout (OOBLECK_REFERENCE), with single-threaded
                          stand-ins (``shims/``) for cppcoro and oneTBB, which this image lacks.  It pins the
                          product's template search and ``get_rank_grid`` (tests/test_planner_vs_reference.py,
                          golden vectors tests/golden/planner.json).  Git-ignored; built by
-                         ``__graft_entry__.build()`` where /root/reference exists.
+                         ``__graft_entry__.build()`` when OOBLECK_REFERENCE is set.
 
 Parity pins: the integer bookkeeping is pinned by golden vectors generated from the
-reference's own Python (tests/golden/gen_golden.py imports /root/reference with the missing
+reference's own Python (tests/golden/gen_golden.py imports the reference checkout with the missing
 third-party modules stubbed) plus the tables of the reference's tests
 (tests/execution/test_reconfiguration.py:151-398, tests/execution/test_engine.py:135-225).
 Floating point: pinned against HF transformers (see above); the deepspeed schedule helper

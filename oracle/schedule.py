@@ -1,7 +1,7 @@
 """Oracle: 1F1B instruction stream.
 
 Restates deepspeed.runtime.pipe.schedule.TrainSchedule helper math (third party, pinned by the
-reference at deepspeed>=0.8.1, environment.yml:29; NOT present under /root/reference -- parity
+reference at deepspeed>=0.8.1, environment.yml:29; NOT present in the reference checkout -- parity
 for the helper math is therefore "unpinned", see oracle/__init__.py) and the reference's own
 override ``OobleckPipelineSchedule.steps`` (oobleck/execution/pipeline.py:34-84).
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate golden vectors for the integer bookkeeping of the hot path FROM THE REFERENCE'S OWN PYTHON.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Run with OOBLECK_REFERENCE naming a checkout of the reference project:
 
     python tests/golden/gen_golden.py        # rewrites tests/golden/*.json
 
@@ -9,7 +9,7 @@ The reference cannot be imported as is (deepspeed, accelerate, pyomo, simple_par
 installed and its C++ planner cannot be built: cppcoro/oneTBB are missing).  This script therefore
 installs *inert stubs* for exactly those third-party modules, then imports the reference's
 ``oobleck.execution.engine`` / ``pipeline`` / ``dataloader`` / ``utils`` modules unmodified from
-/root/reference and drives the real reference functions:
+that checkout and drives the real reference functions:
 
 * ``ReconfigurationEngine.on_reconfigure``      (engine.py:91-180, 311-360)  -> reconfigure.json
 * ``DataParallelEngine.__init__`` grouping      (engine.py:363-398)          -> dp_groups.json
@@ -39,7 +39,7 @@ from unittest.mock import MagicMock
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference"
+REF = os.environ.get("OOBLECK_REFERENCE", "")
 sys.path.insert(0, ROOT)
 sys.path.insert(0, REF)
 

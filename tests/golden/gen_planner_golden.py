@@ -1,12 +1,12 @@
 """Golden vectors for the planner objects from the reference's OWN C++ planner.
 
-    make -C oracle            # builds oracle/_ref/pipeline_template*.so from /root/reference/oobleck/csrc/planning
+    make -C oracle            # builds oracle/_ref/pipeline_template*.so from $OOBLECK_REFERENCE/oobleck/csrc/planning
     python tests/golden/gen_planner_golden.py
 
 Imports the reference's pybind11 module (see oracle/Makefile for how it is built here) and records, for a set of seeded
 random layer profiles, what ``PipelineTemplateGenerator.create_pipeline_templates`` returns (stage splits, GPUs per
 stage, iteration time) and ``PipelineTemplate.get_rank_grid`` of every template -> tests/golden/planner.json.
-The .so cannot travel to a machine without /root/reference being built; the JSON can."""
+The .so needs a checkout of the reference to be built; the JSON does not."""
 import io
 import json
 import os

@@ -229,30 +229,19 @@ def test_measured_profile_feeds_node_range_and_template_search(monkeypatch):
         eng2.instantiate_pipelines(8)
 
 
-_LIVE = {}
-
-
 def live_reference_run():
-    """ONE child process that drives the reference's own classes (tests/golden/gen_golden.py --live: its Python from
-    /root/reference, its C++ planner objects when oracle/_ref is built) on fresh random inputs; shared by the tests below."""
-    import subprocess
-    import sys
-    if not os.path.isdir("/root/reference/oobleck"):
-        pytest.skip("needs /root/reference")
-    if "data" not in _LIVE:
-        r = subprocess.run([sys.executable, os.path.join(G, "gen_golden.py"), "--live", "20260923", "80", "150", "13"],
-                           capture_output=True, text=True, timeout=900)
-        line = next((l for l in reversed(r.stdout.splitlines()) if l.startswith('{"dp_groups"')), None)
-        assert r.returncode == 0 and line is not None, r.stderr[-2000:]
-        _LIVE["data"] = json.loads(line)
-    return _LIVE["data"]
+    """What the reference's own classes computed on seeded random inputs (tests/golden/gen_golden.py --live 20260923 80 150
+    13: its Python, with its own C++ planner objects), stored gzip-compressed as tests/golden/live_reference.json.gz;
+    shared by the tests below."""
+    import gzip
+    with gzip.open(os.path.join(G, "live_reference.json.gz"), "rt") as f:
+        return json.load(f)
 
 
 def test_reconfiguration_policy_live_against_the_reference():
     """Beyond the 120 committed failure sets: 450 fresh ones (up to 13 of the 14 nodes lost, so that "Ranks are
-    insufficient" and the reference's own failure modes occur too) go through the reference's ``on_reconfigure`` in a child
-    process (tests/golden/gen_golden.py --live-reconfigure; the reference's Python with its own C++ planner objects when
-    oracle/_ref is built) and through this package's ``plan_new_ranks``."""
+    insufficient" and the reference's own failure modes occur too) went through the reference's ``on_reconfigure``
+    (stored results, ``live_reference_run``) and go through this package's ``plan_new_ranks``."""
     cases = live_reference_run()["reconfigure"]
     assert len(cases) == 450
     outcomes = {"ranks": 0, "error": 0}
@@ -284,8 +273,8 @@ def test_reconfiguration_policy_live_against_the_reference():
 
 def test_dp_groups_and_sampler_live_against_the_reference():
     """80 random heterogeneous data-parallel layouts through the reference's ``DataParallelEngine.__init__`` (engine.py:
-    363-398) and 80 random sampler configurations through its ``OobleckSampler`` (dataloader.py:13-100), generated in a
-    child process (tests/golden/gen_golden.py --live), against this package's classes."""
+    363-398) and 80 random sampler configurations through its ``OobleckSampler`` (dataloader.py:13-100), stored results
+    (``live_reference_run``), against this package's classes."""
     live = live_reference_run()
     assert len(live["dp_groups"]) == 80 and len(live["sampler"]) == 80
     for c in live["dp_groups"]:
@@ -313,8 +302,8 @@ def test_dp_groups_and_sampler_live_against_the_reference():
 
 def test_pipeline_wiring_live_against_the_reference():
     """The reference's unmodified ``OobleckPipeline.__init__`` / ``initialize_distributed_fsdp`` /
-    ``initialize_distributed_pipeline`` (pipeline.py:431-456, 565-617), run for every rank of 80 random templates in a child
-    process (gen_golden.py --live), against this package's methods of the same names: membership of the pipeline, previous /
+    ``initialize_distributed_pipeline`` (pipeline.py:431-456, 565-617), run for every rank of 80 random templates (stored
+    results, ``live_reference_run``), against this package's methods of the same names: membership of the pipeline, previous /
     next stage rank, per-layer holders, per-shard-column groups in the reference's ``list(set(ranks))`` order.  Templates
     whose stages own different numbers of GPUs are the stated limit (the reference leaves sends without a receiver there,
     pipeline.py:602-610): this package refuses them, and says so."""

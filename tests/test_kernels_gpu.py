@@ -230,8 +230,8 @@ def test_attention_fwd_bwd(B, T, H, h2):
 
 
 def test_attention_lazy_rescale_and_wide_scores():
-    """The forward keeps O in TMEM and moves a row's softmax reference point only when its maximum has grown by more
-    than 2^8 (attention_sm100.cu).  Keys whose norm grows along the sequence force that rescale path many times per
+    """The forward keeps O in registers and moves a row's softmax reference point only when its maximum has grown by
+    more than 2^8 (attention_sm90.cu).  Keys whose norm grows along the sequence force that rescale path many times per
     row; scores spanning +-60 also exercise the exponent range of the fp16-pair probabilities."""
     B, T, H, D = 2, 512, 2, 64
     E = H * D

@@ -112,11 +112,9 @@ def elementwise_report(got, want, name):
 # Elementwise bar (north_star "1e-4 rtol fp32"): |got - ref| <= RTOL * |ref| + ATOL_RMS * rms(ref) for EVERY element,
 # ref = the oracle evaluated in float64, rms over the non-zero reference entries (embedding gradients are mostly exact
 # zeros).  Some absolute floor is needed by ANY fp32 implementation: an entry that is the sum of K products of typical
-# size s carries ~sqrt(K) 2^-24 s of rounding noise however small the entry itself comes out.  Measured on B200 at the
-# GPT-2-XL dims (profiles/r02_stage_parity_xl_dims.log): with a floor of 1e-4 rms the engine has NO violating element
-# in any layer in either backward format, while torch's own fp32 CUDA path (the reference's arithmetic: cuBLAS SGEMM,
-# eager softmax) leaves up to 6e-7 of the elements outside; at 1e-5 rms the engine violates on 1e-6 .. 6e-5 of the
-# elements, torch fp32 on 5e-5 .. 1.5e-3.  The test prints both next to each other.
+# size s carries ~sqrt(K) 2^-24 s of rounding noise however small the entry itself comes out.  At the GPT-2-XL dims the
+# test prints the share of violating elements of the engine next to that of torch's own fp32 CUDA path (the reference's
+# arithmetic: SGEMM, eager softmax) at the same bar.
 ATOL_RMS = 1e-4
 
 

@@ -1,5 +1,5 @@
 """Template search: this repo's planner (csrc/planning/template_search.cpp behind the C ABI) next to the reference's own
-C++ planner (oracle/_ref, built by ``make -C oracle`` from /root/reference/oobleck/csrc/planning with single-threaded
+C++ planner (oracle/_ref, built by ``make -C oracle`` from the reference's oobleck/csrc/planning with single-threaded
 stand-ins for cppcoro / oneTBB), on the same host core, same random layer profile.
 
     python tools/planner_timing.py [layers nodes gpus_per_node [reference_budget_s]]
