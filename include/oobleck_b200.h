@@ -14,12 +14,16 @@
  *     (DESIGN.md "Numerics"): [nplanes][rows][ld] 2-byte elements.  Planes 0-2 are bf16 with x == p0 + p1 + p2 to
  *     24 bits (any range: gradients, everything in backward).  A 5-plane buffer additionally carries, as planes 3-4,
  *     the fp16 pair x ~= h0 + 2^-11 h1 (22 bits, bounded range: weights and forward activations), which needs half
- *     the tensor-core products; producers write all five when asked for nplanes = 5.
+ *     the tensor-core products.
+ *   - every function that writes planes takes the plane set as an `nplanes` code: 1..3 bf16 planes p0..,
+ *     OOB_PLANES_BF16X3_FP16_PAIR or OOB_PLANES_FP16_PAIR.  All of them accept all of these codes, write the same
+ *     bits for the same fp32 value, and reject any other code
  */
 #ifndef OOBLECK_B200_H_
 #define OOBLECK_B200_H_
 
-/* `nplanes` codes understood by every plane producer: 1..3 bf16 planes; 5 = bf16 x 3 + fp16 pair; 22 = fp16 pair only */
+/* plane-set codes besides 1..3: bf16 x 3 followed by the fp16 pair (5 planes); the fp16 pair only, at planes 0-1 */
+#define OOB_PLANES_BF16X3_FP16_PAIR 5
 #define OOB_PLANES_FP16_PAIR 22
 
 #ifdef __cplusplus
@@ -65,7 +69,7 @@ typedef struct oob_gemm_epilogue {
   int accumulate;
   int act;                 /* 0 none, 1 GELU(new): d=pre-activation, planes=gelu;  2 dGELU: value*=gelu'(aux) */
   const float* aux; long ldaux;
-  void* planes; long ldp; long plane_stride; int nplanes_out;   /* 1..3, or 5 (bf16 x 3 + fp16 x 2) */
+  void* planes; long ldp; long plane_stride; int nplanes_out;   /* plane-set code */
   float alpha;
 } oob_gemm_epilogue;
 

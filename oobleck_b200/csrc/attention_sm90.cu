@@ -85,24 +85,6 @@ __device__ __forceinline__ void product(uint32_t sa, uint32_t sb, float (&d)[32]
   for (int i = 0; i < 32; ++i) d[i] = fmaf(c[i], corr_scale<NPL>(), d[i]);
 }
 
-// Two fp32 values -> packed planes (low half = x).
-__device__ __forceinline__ void split_h2_x2(float x, float y, uint32_t& h0, uint32_t& h1) {
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h0) : "f"(y), "f"(x));
-  float fx, fy;
-  asm("{\n\t.reg .f16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\tcvt.f32.f16 %0, lo;\n\tcvt.f32.f16 %1, hi;\n\t}"
-      : "=f"(fx), "=f"(fy)
-      : "r"(h0));
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h1) : "f"((y - fy) * H1_SCALE), "f"((x - fx) * H1_SCALE));
-}
-__device__ __forceinline__ void split3_x2(float x, float y, uint32_t& p0, uint32_t& p1, uint32_t& p2) {
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p0) : "f"(y), "f"(x));
-  float rx = x - __uint_as_float(p0 << 16), ry = y - __uint_as_float(p0 & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p1) : "f"(ry), "f"(rx));
-  rx -= __uint_as_float(p1 << 16);
-  ry -= __uint_as_float(p1 & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p2) : "f"(ry), "f"(rx));
-}
-
 // The accumulator fragment d (32 values per thread) -> the planes of a thread-written A tile (K-major,
 // SWIZZLE_128B: the 16-byte chunk index is XORed with row & 7 -- the pattern TMA produces for the loaded tiles)
 template <int NPL>
@@ -126,34 +108,19 @@ __device__ __forceinline__ void store_tile(uint32_t s_tile, int warp, int lane, 
   }
 }
 
-// 2 consecutive output elements: fp32 and / or split planes (plane-set codes of common.cuh)
-__device__ __forceinline__ void store_pair(float* f32, uint16_t* planes, long ps, int code, long off, float x, float y) {
-  if (f32) *reinterpret_cast<float2*>(f32 + off) = make_float2(x, y);
-  if (!planes) return;
-  uint16_t* pp = planes + off;
-  if (code != PLANES_H2) {
-    uint32_t p0, p1, p2;
-    split3_x2(x, y, p0, p1, p2);
-    *reinterpret_cast<uint32_t*>(pp) = p0;
-    if (code > 1) *reinterpret_cast<uint32_t*>(pp + ps) = p1;
-    if (code > 2) *reinterpret_cast<uint32_t*>(pp + 2 * ps) = p2;
-  }
-  if (code == 5 || code == PLANES_H2) {
-    uint32_t h0, h1;
-    split_h2_x2(x, y, h0, h1);
-    uint16_t* ph = code == 5 ? pp + 3 * ps : pp;
-    *reinterpret_cast<uint32_t*>(ph) = h0;
-    *reinterpret_cast<uint32_t*>(ph + ps) = h1;
-  }
-}
-
-// rows [grow0, grow0 + rows_valid) x 64 columns starting at element offset col0 of a [*, ld] matrix, from a fragment
+// rows [grow0, grow0 + rows_valid) x 64 columns starting at element offset col0 of a [*, ld] matrix, from a fragment:
+// fp32 and / or the planes of `code`
 __device__ __forceinline__ void store_fragment(const float (&v)[32], int warp, int lane, float* f32, uint16_t* planes,
                                                long ps, int code, long grow0, int rows_valid, long ld, long col0) {
 #pragma unroll
   for (int i = 0; i < 32; i += 2) {
     const int row = frag_row(warp, lane, i);
-    if (row < rows_valid) store_pair(f32, planes, ps, code, (grow0 + row) * ld + col0 + frag_col(lane, i), v[i], v[i + 1]);
+    if (row < rows_valid) {
+      const long off = (grow0 + row) * ld + col0 + frag_col(lane, i);
+      const float e[2] = {v[i], v[i + 1]};
+      if (f32) *reinterpret_cast<float2*>(f32 + off) = make_float2(e[0], e[1]);
+      if (planes) store_planes(planes + off, ps, code, e);
+    }
   }
 }
 
@@ -553,6 +520,7 @@ int attention_fwd(const bf16* qkv_planes, long qkv_plane_stride, int operand_fp1
                   long plane_stride, int nplanes, float* lse, int B, int T, int H, int D, cudaStream_t s) {
   OOB_CHECK(D == AD, "attention: head_dim must be 64 (got %d)", D);
   OOB_CHECK(B > 0 && T > 0 && H > 0, "attention: empty problem");
+  OOB_CHECK(!out_planes || planes_code_valid(nplanes), "attention: unknown plane-set code %d", nplanes);
   return operand_fp16 ? attention_fwd_t<2>(qkv_planes, qkv_plane_stride, out, out_planes, plane_stride, nplanes, lse, B,
                                            T, H, s)
                       : attention_fwd_t<3>(qkv_planes, qkv_plane_stride, out, out_planes, plane_stride, nplanes, lse, B,
@@ -564,6 +532,7 @@ int attention_bwd(const bf16* qkv_planes, long qkv_plane_stride, int operand_fp1
                   bf16* dqkv_planes, long plane_stride, int nplanes, int B, int T, int H, int D, cudaStream_t s) {
   OOB_CHECK(D == AD, "attention: head_dim must be 64 (got %d)", D);
   OOB_CHECK(B > 0 && T > 0 && H > 0, "attention: empty problem");
+  OOB_CHECK(!dqkv_planes || planes_code_valid(nplanes), "attention: unknown plane-set code %d", nplanes);
   return operand_fp16 ? attention_bwd_t<2>(qkv_planes, qkv_plane_stride, out, dout, dout_planes, dout_plane_stride, lse,
                                            delta, dqkv, dqkv_planes, plane_stride, nplanes, B, T, H, s)
                       : attention_bwd_t<3>(qkv_planes, qkv_plane_stride, out, dout, dout_planes, dout_plane_stride, lse,

@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/oobleck_b200.h"
+
 namespace oob {
 
 // ---------------------------------------------------------------------------------------------
@@ -38,14 +40,6 @@ void count_launch(int n = 1);
 //   nsplit 3: + p1q1 + p0q2 + p2q0      (~2^-23, fp32-grade, 6 MMAs)   <- parity mode
 typedef __nv_bfloat16 bf16;
 
-__device__ __forceinline__ void split3(float x, bf16& p0, bf16& p1, bf16& p2) {
-  p0 = __float2bfloat16_rn(x);
-  float r = x - __bfloat162float(p0);
-  p1 = __float2bfloat16_rn(r);
-  r -= __bfloat162float(p1);
-  p2 = __float2bfloat16_rn(r);
-}
-
 // Second operand format: TWO fp16 planes, x ~= h0 + 2^-11 * h1 with h0 = fp16(x), h1 = fp16((x - h0) * 2^11).
 // 22 significand bits (fp16 carries 11 per plane; the residual is pre-scaled so it never falls into fp16 subnormals
 // before x itself is below ~2^-14), so the three products h0g0 + 2^-11 (h0g1 + h1g0) are fp32-grade at half the
@@ -54,26 +48,62 @@ __device__ __forceinline__ void split3(float x, bf16& p0, bf16& p1, bf16& p2) {
 // Conversions saturate (no inf) so an outlier degrades precision instead of poisoning the GEMM.
 constexpr float H1_SCALE = 2048.f;
 constexpr float H1_INV_SCALE = 1.f / 2048.f;
-__device__ __forceinline__ uint16_t f2h_sat(float x) {
-  uint16_t h;
-  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
-  return h;
+
+// Both splits of two fp32 values at once: one 32-bit word per plane, x in the low half.  The packed conversions round
+// like their scalar forms, so an element's planes depend on that element alone.
+__device__ __forceinline__ void split3_x2(float x, float y, uint32_t& p0, uint32_t& p1, uint32_t& p2) {
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p0) : "f"(y), "f"(x));
+  float rx = x - __uint_as_float(p0 << 16), ry = y - __uint_as_float(p0 & 0xffff0000u);
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p1) : "f"(ry), "f"(rx));
+  rx -= __uint_as_float(p1 << 16);
+  ry -= __uint_as_float(p1 & 0xffff0000u);
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p2) : "f"(ry), "f"(rx));
 }
-__device__ __forceinline__ float h2f(uint16_t h) {
-  float f;
-  asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
-  return f;
+__device__ __forceinline__ void split_h2_x2(float x, float y, uint32_t& h0, uint32_t& h1) {
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h0) : "f"(y), "f"(x));
+  float fx, fy;
+  asm("{\n\t.reg .f16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\tcvt.f32.f16 %0, lo;\n\tcvt.f32.f16 %1, hi;\n\t}"
+      : "=f"(fx), "=f"(fy)
+      : "r"(h0));
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h1) : "f"((y - fy) * H1_SCALE), "f"((x - fx) * H1_SCALE));
 }
-__device__ __forceinline__ void split_h2(float x, uint16_t& h0, uint16_t& h1) {
-  h0 = f2h_sat(x);
-  h1 = f2h_sat((x - h2f(h0)) * H1_SCALE);
+
+// Plane-set codes (include/oobleck_b200.h): which planes a producer writes.
+//   1..3                          bf16 planes p0..  (x = p0 + p1 + p2)
+//   OOB_PLANES_BF16X3_FP16_PAIR   bf16 x 3 followed by the fp16 pair
+//   OOB_PLANES_FP16_PAIR          the fp16 pair only, at planes 0 and 1 (loss-scaled gradients, backward GEMM operands)
+__host__ __device__ __forceinline__ int planes_count(int code) { return code == OOB_PLANES_FP16_PAIR ? 2 : code; }
+inline bool planes_code_valid(int code) {
+  return (code >= 1 && code <= 3) || code == OOB_PLANES_BF16X3_FP16_PAIR || code == OOB_PLANES_FP16_PAIR;
 }
-// raw 16-bit patterns of all five planes of a "5-plane" buffer: [bf16 p0 p1 p2 | fp16 h0 h1]
-__device__ __forceinline__ void split5(float x, uint16_t& q0, uint16_t& q1, uint16_t& q2, uint16_t& q3, uint16_t& q4) {
-  bf16 a, b, c;
-  split3(x, a, b, c);
-  q0 = __bfloat16_as_ushort(a); q1 = __bfloat16_as_ushort(b); q2 = __bfloat16_as_ushort(c);
-  split_h2(x, q3, q4);
+
+template <int N>
+__device__ __forceinline__ void store_plane(uint16_t* p, const uint32_t (&w)[(N + 1) / 2]) {
+  if constexpr (N == 4) *reinterpret_cast<uint2*>(p) = make_uint2(w[0], w[1]);
+  else if constexpr (N == 2) *reinterpret_cast<uint32_t*>(p) = w[0];
+  else *p = (uint16_t)w[0];
+}
+// The plane writer: N consecutive values v into the planes of `code`, plane i at p + i * plane_stride.  N = 4 or 2 is
+// one 8- or 4-byte store per plane (p aligned to it); N = 1 is the per-element form for ragged edges and tails.
+template <int N>
+__device__ __forceinline__ void store_planes(uint16_t* p, long plane_stride, int code, const float (&v)[N]) {
+  static_assert(N == 1 || N == 2 || N == 4, "1, 2 or 4 consecutive values");
+  constexpr int W = (N + 1) / 2;
+  if (code != OOB_PLANES_FP16_PAIR) {
+    uint32_t b0[W], b1[W], b2[W];
+#pragma unroll
+    for (int j = 0; j < W; ++j) split3_x2(v[2 * j], v[N == 1 ? 0 : 2 * j + 1], b0[j], b1[j], b2[j]);
+    store_plane<N>(p, b0);
+    if (code > 1) store_plane<N>(p + plane_stride, b1);
+    if (code > 2) store_plane<N>(p + 2 * plane_stride, b2);
+    if (code != OOB_PLANES_BF16X3_FP16_PAIR) return;
+    p += 3 * plane_stride;   // the fp16 pair follows the bf16 planes
+  }
+  uint32_t h0[W], h1[W];
+#pragma unroll
+  for (int j = 0; j < W; ++j) split_h2_x2(v[2 * j], v[N == 1 ? 0 : 2 * j + 1], h0[j], h1[j]);
+  store_plane<N>(p, h0);
+  store_plane<N>(p + plane_stride, h1);
 }
 
 // tanh(u) = 1 - 2 / (1 + e^{2u}) on the SFU (ex2 + rcp, ~2 ulp each; saturates correctly at +-inf).  The libm
@@ -82,15 +112,6 @@ __device__ __forceinline__ void split5(float x, uint16_t& q0, uint16_t& q1, uint
 __device__ __forceinline__ float tanh_fast(float u) {
   return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * u));
 }
-// Plane-set codes accepted by every producer's `nplanes` argument:
-//   1..3        bf16 planes p0..  (x = p0 + p1 + p2)
-//   5           bf16 x 3 followed by the fp16 pair
-//   PLANES_H2   the fp16 pair only, at planes 0 and 1 (loss-scaled gradients, backward GEMM operands)
-constexpr int PLANES_H2 = 22;
-__host__ __device__ __forceinline__ int planes_count(int code) { return code == PLANES_H2 ? 2 : code; }
-// which of split5's five outputs goes to stored plane i
-__host__ __device__ __forceinline__ int planes_src(int code, int i) { return code == PLANES_H2 ? 3 + i : i; }
-
 __device__ __forceinline__ float gelu_new_f(float x) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
   float u = k0 * (x + k1 * x * x * x);

@@ -11,33 +11,16 @@ __global__ void split_kernel(const float* __restrict__ x, bf16* __restrict__ pla
                              int nplanes) {
   long i = ((long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const long step = (long)gridDim.x * blockDim.x * 4;
+  uint16_t* const out = reinterpret_cast<uint16_t*>(planes);
   for (; i < n; i += step) {
-    float v[4];
     if (i + 4 <= n) {
-      float4 t = ldg_f4(x + i);
-      v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+      const float4 t = ldg_f4(x + i);
+      const float v[4] = {t.x, t.y, t.z, t.w};
+      store_planes(out + i, plane_stride, nplanes, v);
     } else {
-      for (int j = 0; j < 4; ++j) v[j] = (i + j < n) ? x[i + j] : 0.f;
-    }
-    uint16_t q[5][4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) split5(v[j], q[0][j], q[1][j], q[2][j], q[3][j], q[4][j]);
-    const bool h2 = nplanes == PLANES_H2;
-    const int cnt = planes_count(nplanes);
-#pragma unroll
-    for (int p = 0; p < 5; ++p) {
-      if (p >= cnt) break;
-      uint16_t* dst = reinterpret_cast<uint16_t*>(planes) + p * plane_stride + i;
-      uint16_t v4[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) v4[j] = (h2 && p < 2) ? q[3 + (p & 1)][j] : q[p][j];
-      if (i + 4 <= n) {
-        uint2 w;
-        w.x = (uint32_t)v4[0] | ((uint32_t)v4[1] << 16);
-        w.y = (uint32_t)v4[2] | ((uint32_t)v4[3] << 16);
-        *reinterpret_cast<uint2*>(dst) = w;
-      } else {
-        for (int j = 0; j < 4 && i + j < n; ++j) dst[j] = v4[j];
+      for (long j = i; j < n; ++j) {
+        const float v[1] = {x[j]};
+        store_planes(out + j, plane_stride, nplanes, v);
       }
     }
   }
@@ -47,6 +30,7 @@ int split_planes(const float* x, bf16* planes, long n, long plane_stride, int np
   OOB_CHECK((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(planes) & 7) == 0 &&
                 (plane_stride & 3) == 0,
             "split_planes: misaligned buffers");
+  OOB_CHECK(planes_code_valid(nplanes), "split_planes: unknown plane-set code %d", nplanes);
   if (n <= 0) return 0;
   int blocks = (int)((n / 4 + 255) / 256);
   if (blocks > 132 * 8) blocks = 132 * 8;
@@ -103,27 +87,7 @@ layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamm
       float o[4] = {(v[i].x - mu) * rs * g.x + b.x, (v[i].y - mu) * rs * g.y + b.y, (v[i].z - mu) * rs * g.z + b.z,
                     (v[i].w - mu) * rs * g.w + b.w};
       if (y) stg_f4(y + (long)row * E + c * 4, make_float4(o[0], o[1], o[2], o[3]));
-      if (planes) {
-        uint16_t pq[5][4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) split5(o[j], pq[0][j], pq[1][j], pq[2][j], pq[3][j], pq[4][j]);
-        const bool h2 = nplanes == PLANES_H2;
-        const int cnt = planes_count(nplanes);
-#pragma unroll
-        for (int p = 0; p < 5; ++p) {
-          if (p < cnt) {
-            uint2 w;   // pair-only buffers carry h0, h1 at planes 0, 1
-            if (h2 && p < 2) {
-              w.x = (uint32_t)pq[3 + (p & 1)][0] | ((uint32_t)pq[3 + (p & 1)][1] << 16);
-              w.y = (uint32_t)pq[3 + (p & 1)][2] | ((uint32_t)pq[3 + (p & 1)][3] << 16);
-            } else {
-              w.x = (uint32_t)pq[p][0] | ((uint32_t)pq[p][1] << 16);
-              w.y = (uint32_t)pq[p][2] | ((uint32_t)pq[p][3] << 16);
-            }
-            *reinterpret_cast<uint2*>(planes + p * plane_stride + (long)row * E + c * 4) = w;
-          }
-        }
-      }
+      if (planes) store_planes(reinterpret_cast<uint16_t*>(planes) + (long)row * E + c * 4, plane_stride, nplanes, o);
     }
   }
 }
@@ -131,6 +95,7 @@ layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamm
 int layernorm_fwd(const float* x, const float* gamma, const float* beta, float* y, bf16* planes, long plane_stride,
                   int nplanes, float* mean, float* rstd, int rows, int E, float eps, cudaStream_t s) {
   OOB_CHECK(E % 4 == 0 && E <= LN_MAXV * 128, "layernorm: E=%d unsupported (need E%%4==0, E<=%d)", E, LN_MAXV * 128);
+  OOB_CHECK(!planes || planes_code_valid(nplanes), "layernorm: unknown plane-set code %d", nplanes);
   if (rows <= 0) return 0;
   layernorm_fwd_kernel<<<(rows + 3) / 4, 128, 0, s>>>(x, gamma, beta, y, planes, plane_stride, nplanes, mean, rstd,
                                                       rows, E, eps);
@@ -146,12 +111,18 @@ int layernorm_fwd(const float* x, const float* gamma, const float* beta, float* 
 // `partials` ([grid][2][E]); colreduce_finalize folds them into the flat gradient in a fixed order.
 constexpr int LNB_V = 2;  // float4 columns per thread (E <= 2048)
 
+// PAIR5: the instance for OOB_PLANES_BF16X3_FP16_PAIR.  Writing both plane families keeps the output live across all
+// five stores and costs 13 registers, which would leave room for 3 instead of 4 CTAs per SM (LN_BWD_MAX_GRID); the
+// stage writes gradients as bf16 x 3 or as the pair only, so it runs the other instance.
+template <bool PAIR5>
 __global__ void __launch_bounds__(256)
 layernorm_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
                      const float* __restrict__ rstd, const float* __restrict__ gamma, const float* __restrict__ dres,
                      float* __restrict__ dx, bf16* __restrict__ planes, long plane_stride, int nplanes,
                      float* __restrict__ partials, int rows, int E) {
   __shared__ float sh[2][8];
+  // the launcher passes OOB_PLANES_BF16X3_FP16_PAIR to PAIR5 only: the other instance compiles without that path
+  const int code = PAIR5 ? OOB_PLANES_BF16X3_FP16_PAIR : (nplanes == OOB_PLANES_BF16X3_FP16_PAIR ? 3 : nplanes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nv = E >> 2;
   float4 ag[LNB_V], ab[LNB_V], gm[LNB_V];
@@ -202,30 +173,7 @@ layernorm_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, 
           o[0] += r.x; o[1] += r.y; o[2] += r.z; o[3] += r.w;
         }
         if (dx) stg_f4(dx + (long)row * E + c * 4, make_float4(o[0], o[1], o[2], o[3]));
-        if (planes) {
-          if (nplanes == PLANES_H2) {   // loss-scaled gradient: fp16 pair only
-            uint16_t h0[4], h1[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) split_h2(o[j], h0[j], h1[j]);
-            *reinterpret_cast<uint2*>(planes + (long)row * E + c * 4) =
-                make_uint2((uint32_t)h0[0] | ((uint32_t)h0[1] << 16), (uint32_t)h0[2] | ((uint32_t)h0[3] << 16));
-            *reinterpret_cast<uint2*>(planes + plane_stride + (long)row * E + c * 4) =
-                make_uint2((uint32_t)h1[0] | ((uint32_t)h1[1] << 16), (uint32_t)h1[2] | ((uint32_t)h1[3] << 16));
-          } else {
-            bf16 pq[3][4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) split3(o[j], pq[0][j], pq[1][j], pq[2][j]);
-#pragma unroll
-            for (int p = 0; p < 3; ++p) {
-              if (p < nplanes) {
-                uint2 w;
-                w.x = (uint32_t)__bfloat16_as_ushort(pq[p][0]) | ((uint32_t)__bfloat16_as_ushort(pq[p][1]) << 16);
-                w.y = (uint32_t)__bfloat16_as_ushort(pq[p][2]) | ((uint32_t)__bfloat16_as_ushort(pq[p][3]) << 16);
-                *reinterpret_cast<uint2*>(planes + p * plane_stride + (long)row * E + c * 4) = w;
-              }
-            }
-          }
-        }
+        if (planes) store_planes(reinterpret_cast<uint16_t*>(planes) + (long)row * E + c * 4, plane_stride, code, o);
       }
     }
   }
@@ -265,10 +213,11 @@ int layernorm_bwd(const float* dy, const float* x, const float* mean, const floa
                   const float* dres, float* dx, bf16* planes, long plane_stride, int nplanes, float* dgamma,
                   float* dbeta, float* partials, int rows, int E, float gscale, cudaStream_t s) {
   OOB_CHECK(E % 4 == 0 && E <= LNB_V * 256 * 4, "layernorm_bwd: E=%d unsupported", E);
+  OOB_CHECK(!planes || planes_code_valid(nplanes), "layernorm_bwd: unknown plane-set code %d", nplanes);
   if (rows <= 0) return 0;
   int grid = rows < LN_BWD_MAX_GRID ? rows : LN_BWD_MAX_GRID;
-  layernorm_bwd_kernel<<<grid, 256, 0, s>>>(dy, x, mean, rstd, gamma, dres, dx, planes, plane_stride, nplanes,
-                                            partials, rows, E);
+  auto kernel = nplanes == OOB_PLANES_BF16X3_FP16_PAIR ? layernorm_bwd_kernel<true> : layernorm_bwd_kernel<false>;
+  kernel<<<grid, 256, 0, s>>>(dy, x, mean, rstd, gamma, dres, dx, planes, plane_stride, nplanes, partials, rows, E);
   OOB_CUDA_OK(cudaGetLastError());
   count_launch();
   colreduce_finalize_kernel<<<(2 * E + 31) / 32, dim3(32, 8), 0, s>>>(partials, grid, 2 * E, dgamma, dbeta, E, gscale);
@@ -463,21 +412,7 @@ cross_entropy_kernel(const float* __restrict__ logits, long ldl, const long long
         g[j] = 0.f;
         if (cc < V) g[j] = (expf(lr[cc] - mx) * inv - (cc == target ? 1.f : 0.f)) * grad_scale;
       }
-      if (nplanes == PLANES_H2) {
-        uint16_t a0, a1, b0, b1;
-        split_h2(g[0], a0, a1);
-        split_h2(g[1], b0, b1);
-        *reinterpret_cast<uint32_t*>(dplanes + (long)row * ldp + c) = (uint32_t)a0 | ((uint32_t)b0 << 16);
-        *reinterpret_cast<uint32_t*>(dplanes + plane_stride + (long)row * ldp + c) = (uint32_t)a1 | ((uint32_t)b1 << 16);
-      } else {
-        bf16 a[3], b[3];
-        split3(g[0], a[0], a[1], a[2]);
-        split3(g[1], b[0], b[1], b[2]);
-        for (int p = 0; p < nplanes; ++p) {
-          const uint32_t w = (uint32_t)__bfloat16_as_ushort(a[p]) | ((uint32_t)__bfloat16_as_ushort(b[p]) << 16);
-          *reinterpret_cast<uint32_t*>(dplanes + p * plane_stride + (long)row * ldp + c) = w;
-        }
-      }
+      store_planes(reinterpret_cast<uint16_t*>(dplanes) + (long)row * ldp + c, plane_stride, nplanes, g);
     }
   }
 }
@@ -505,6 +440,7 @@ int cross_entropy(const float* logits, long ldl, const long long* labels, int B,
   const int rows = B * T;
   OOB_CHECK(T >= 2, "cross_entropy: sequence length must be >= 2");
   OOB_CHECK(dplanes == nullptr || (ldp % 8 == 0 && plane_stride % 8 == 0), "cross_entropy: plane strides must be multiples of 8");
+  OOB_CHECK(!dplanes || planes_code_valid(nplanes), "cross_entropy: unknown plane-set code %d", nplanes);
   cross_entropy_kernel<<<rows, 512, 0, s>>>(logits, ldl, labels, rows, T, V, grad_scale, row_loss, dplanes, ldp,
                                             plane_stride, nplanes);
   OOB_CUDA_OK(cudaGetLastError());
@@ -554,25 +490,13 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
       for (int j = 0; j < 4 && i + j < n; ++j) { p[i + j] = pv[j]; m[i + j] = mv[j]; v[i + j] = vv[j]; }
     }
     if (planes) {
-      uint16_t q[5][4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) split5(pv[j], q[0][j], q[1][j], q[2][j], q[3][j], q[4][j]);
-      const bool h2 = nplanes == PLANES_H2;
-      const int cnt = planes_count(nplanes);
-#pragma unroll
-      for (int pl = 0; pl < 5; ++pl) {
-        if (pl >= cnt) break;
-        uint16_t* dst = reinterpret_cast<uint16_t*>(planes) + pl * plane_stride + i;
-        uint16_t v4[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) v4[j] = (h2 && pl < 2) ? q[3 + (pl & 1)][j] : q[pl][j];
-        if (full) {
-          uint2 w;
-          w.x = (uint32_t)v4[0] | ((uint32_t)v4[1] << 16);
-          w.y = (uint32_t)v4[2] | ((uint32_t)v4[3] << 16);
-          *reinterpret_cast<uint2*>(dst) = w;
-        } else {
-          for (int j = 0; j < 4 && i + j < n; ++j) dst[j] = v4[j];
+      uint16_t* const dst = reinterpret_cast<uint16_t*>(planes) + i;
+      if (full) {
+        store_planes(dst, plane_stride, nplanes, pv);
+      } else {
+        for (int j = 0; j < 4 && i + j < n; ++j) {
+          const float e[1] = {pv[j]};
+          store_planes(dst + j, plane_stride, nplanes, e);
         }
       }
     }
@@ -583,6 +507,7 @@ int adamw_step(float* p, const float* g, float* m, float* v, bf16* planes, long 
                float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t s) {
   if (n <= 0) return 0;
   OOB_CHECK(step >= 1, "adamw: step is 1-based");
+  OOB_CHECK(!planes || planes_code_valid(nplanes), "adamw: unknown plane-set code %d", nplanes);
   const double bc1 = 1.0 - pow((double)beta1, step);
   const double bc2 = 1.0 - pow((double)beta2, step);
   long blocks = (n / 4 + 255) / 256;

@@ -159,6 +159,7 @@ int gemm_launch(const PlaneMat& A, int a_mn, const PlaneMat& B, int b_mn, const 
     if (p.nsplit == 2) p.corr_scale = 1.0f / 2048.0f;
   }
   OOB_CHECK(A.nplanes >= p.nsplit && B.nplanes >= p.nsplit, "operands carry fewer planes than nsplit");
+  OOB_CHECK(!p.epi.planes || planes_code_valid(p.epi.nplanes_out), "GEMM: unknown plane-set code %d", p.epi.nplanes_out);
   {
     GemmEpilogue& e = p.epi;
     auto ok16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };

@@ -39,7 +39,7 @@ struct GemmEpilogue {
   bf16* planes;         // split output [nplanes_out][M][ldp] or null
   long ldp;
   long plane_stride;
-  int nplanes_out;      // plane-set code (common.cuh): 1..3 bf16 planes, 5 = bf16 x 3 + fp16 pair, PLANES_H2 = pair only
+  int nplanes_out;      // plane-set code (common.cuh)
   float alpha;          // value = alpha * acc (before bias etc.)
   int vec4;             // set by gemm_launch: every pointer / stride above allows 16-B (fp32) and 8-B (plane) accesses
 };
@@ -68,10 +68,6 @@ constexpr int GEMM_CHUNK_ELEMS = 512;
 
 __host__ __device__ constexpr int gemm_stage_bytes(int nsplit) { return nsplit * (GEMM_BM + GEMM_BN) * GEMM_BK * 2; }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(bf16 lo, bf16 hi) {
-  return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
-}
-
 // The fused epilogue of 4 consecutive output elements (row grow, columns gcol ..) with accumulator values v.
 __device__ __forceinline__ void epilogue_quad(const GemmEpilogue& ep, long grow, int gcol, int N, float4 v) {
   float* const d = ep.d;
@@ -91,13 +87,8 @@ __device__ __forceinline__ void epilogue_quad(const GemmEpilogue& ep, long grow,
       if (act == ACT_DGELU) y *= gelu_new_grad_f(ep.aux[grow * ep.ldaux + gcol + j]);
       if (d) d[grow * ep.ldd + gcol + j] = y;
       if (planes) {
-        if (act == ACT_GELU) y = gelu_new_f(y);
-        uint16_t w[5];
-        split5(y, w[0], w[1], w[2], w[3], w[4]);
-#pragma unroll
-        for (int pl = 0; pl < 5; ++pl)
-          if (pl < planes_count(nplanes_out))
-            planes[pl * pstride + grow * ep.ldp + gcol + j] = (nplanes_out == PLANES_H2 && pl < 2) ? w[3 + (pl & 1)] : w[pl];
+        const float e[1] = {act == ACT_GELU ? gelu_new_f(y) : y};
+        store_planes(planes + grow * ep.ldp + gcol + j, pstride, nplanes_out, e);
       }
     }
     return;
@@ -119,27 +110,7 @@ __device__ __forceinline__ void epilogue_quad(const GemmEpilogue& ep, long grow,
 #pragma unroll
       for (int j = 0; j < 4; ++j) y[j] = gelu_new_f(y[j]);
     }
-    uint16_t* pp = planes + grow * ep.ldp + gcol;
-    if (nplanes_out <= 3 || nplanes_out == 5) {
-      bf16 p0[4], p1[4], p2[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) split3(y[j], p0[j], p1[j], p2[j]);
-      *reinterpret_cast<uint2*>(pp) = make_uint2(pack_bf16x2(p0[0], p0[1]), pack_bf16x2(p0[2], p0[3]));
-      if (nplanes_out > 1)
-        *reinterpret_cast<uint2*>(pp + pstride) = make_uint2(pack_bf16x2(p1[0], p1[1]), pack_bf16x2(p1[2], p1[3]));
-      if (nplanes_out > 2)
-        *reinterpret_cast<uint2*>(pp + 2 * pstride) = make_uint2(pack_bf16x2(p2[0], p2[1]), pack_bf16x2(p2[2], p2[3]));
-    }
-    if (nplanes_out == 5 || nplanes_out == PLANES_H2) {
-      uint16_t h0[4], h1[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) split_h2(y[j], h0[j], h1[j]);
-      uint16_t* ph = nplanes_out == 5 ? pp + 3 * pstride : pp;
-      *reinterpret_cast<uint2*>(ph) =
-          make_uint2((uint32_t)h0[0] | ((uint32_t)h0[1] << 16), (uint32_t)h0[2] | ((uint32_t)h0[3] << 16));
-      *reinterpret_cast<uint2*>(ph + pstride) =
-          make_uint2((uint32_t)h1[0] | ((uint32_t)h1[1] << 16), (uint32_t)h1[2] | ((uint32_t)h1[3] << 16));
-    }
+    store_planes(planes + grow * ep.ldp + gcol, pstride, nplanes_out, y);
   }
 }
 

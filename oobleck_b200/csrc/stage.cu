@@ -29,26 +29,45 @@ struct BlockOffsets {  // element offsets inside the flat parameter vector, HF G
   }
 };
 
-inline PlaneMat weight_planes(const oob_layer_params* p, long off, long rows, long cols) {
-  return PlaneMat{reinterpret_cast<const bf16*>(p->w_planes) + off, rows, cols, cols, p->plane_stride, 3};
+// The planes of a buffer a GEMM reads: `nplanes` planes from plane `first` on, bf16 planes or an fp16 pair.
+struct PlaneView {
+  int first, nplanes, fp16;
+  PlaneMat of(const void* base, long rows, long cols, long plane_stride) const {
+    return PlaneMat{reinterpret_cast<const bf16*>(base) + first * plane_stride, rows, cols, cols, plane_stride, nplanes,
+                    fp16};
+  }
+  PlaneMat act(const void* base, long rows, long cols) const { return of(base, rows, cols, rows * cols); }
+  PlaneMat weight(const oob_layer_params* p, long off, long rows, long cols) const {
+    return of(reinterpret_cast<const bf16*>(p->w_planes) + off, rows, cols, p->plane_stride);
+  }
+};
+
+// Operand formats of a stage call, all decided by oob_dims.fwd_fp16 / bwd_fp16 / nsplit (include/oobleck_b200.h).
+struct Formats {
+  int act_code;      // weights and every saved activation a GEMM reads: bf16 x 3, + fp16 pair, or the pair only
+  int qkv_code;      // q|k|v, whose only reader is attention
+  int grad_code;     // activation gradients
+  int attn_fp16;     // attention reads q|k|v and dO as fp16 pairs
+  int fwd_nsplit, bwd_nsplit;
+  float unscale;     // 1 / loss scale of the activation gradients: applied where parameter gradients are produced
+  PlaneView fwd;     // what a forward GEMM reads of an activation or a weight buffer
+  PlaneView bwd;     // what a dgrad / wgrad reads of a gradient, a saved activation or a weight buffer
+};
+Formats formats(const oob_dims* d) {
+  const bool h = d->fwd_fp16 != 0, hb = d->bwd_fp16 != 0;
+  const PlaneView bf16x3{0, 3, 0}, pair_at0{0, 2, 1}, pair_at3{3, 2, 1};
+  Formats f;
+  f.act_code = hb ? OOB_PLANES_FP16_PAIR : (h ? OOB_PLANES_BF16X3_FP16_PAIR : 3);
+  f.qkv_code = f.grad_code = hb ? OOB_PLANES_FP16_PAIR : 3;
+  f.attn_fp16 = hb ? 1 : 0;
+  f.fwd_nsplit = h ? 2 : d->nsplit;
+  f.bwd_nsplit = hb ? 2 : d->nsplit;
+  f.unscale = hb ? 1.0f / d->loss_scale : 1.0f;
+  f.fwd = h ? (hb ? pair_at0 : pair_at3) : bf16x3;
+  f.bwd = hb ? pair_at0 : bf16x3;
+  return f;
 }
-inline PlaneMat act_planes(const void* base, long rows, long cols) {
-  return PlaneMat{reinterpret_cast<const bf16*>(base), rows, cols, cols, rows * cols, 3};
-}
-// the fp16 x 2 pair of a 5-plane buffer (planes 3, 4): forward-GEMM operands when oob_dims.fwd_fp16 is set
-// `at0`: the buffer is pair-only (PLANES_H2, all-fp16 mode) and the pair sits at planes 0, 1
-inline PlaneMat weight_planes_h(const oob_layer_params* p, long off, long rows, long cols, bool at0) {
-  return PlaneMat{reinterpret_cast<const bf16*>(p->w_planes) + (at0 ? 0 : 3) * p->plane_stride + off, rows, cols, cols,
-                  p->plane_stride, 2, 1};
-}
-inline PlaneMat act_planes_h(const void* base, long rows, long cols, bool at0) {
-  return PlaneMat{reinterpret_cast<const bf16*>(base) + (at0 ? 0 : 3) * rows * cols, rows, cols, cols, rows * cols, 2,
-                  1};
-}
-// a loss-scaled gradient stored as an fp16 pair at planes 0, 1 (bwd_fp16 mode)
-inline PlaneMat grad_planes_h(const void* base, long rows, long cols) {
-  return PlaneMat{reinterpret_cast<const bf16*>(base), rows, cols, cols, rows * cols, 2, 1};
-}
+
 inline GemmEpilogue epi_none() {
   GemmEpilogue e{};
   e.alpha = 1.0f;
@@ -56,12 +75,10 @@ inline GemmEpilogue epi_none() {
 }
 
 // D = A[M,K] . W[K,N] + bias (+resid); optionally the split planes of the result (or of GELU(result))
-// `a_base` is the input's plane buffer: bf16 x 3, or 5 planes when fp16_ops (then the fp16 pair is the operand and the
-// weights' fp16 pair is used: 3 tensor-core products instead of 6)
-int linear_fwd(const void* a_base, bool fp16_ops, bool at0, const oob_layer_params* p, long w_off, long b_off, int M, int N,
-               int K, int nsplit, float* d, const float* resid, bf16* planes_out, int nplanes_out, bool gelu,
-               cudaStream_t st) {
-  GemmParams gp{M, N, K, fp16_ops ? 2 : nsplit, epi_none()};
+// `a_base` is the input's plane buffer
+int linear_fwd(const Formats& f, const void* a_base, const oob_layer_params* p, long w_off, long b_off, int M, int N,
+               int K, float* d, const float* resid, bf16* planes_out, int nplanes_out, bool gelu, cudaStream_t st) {
+  GemmParams gp{M, N, K, f.fwd_nsplit, epi_none()};
   gp.epi.d = d; gp.epi.ldd = N;
   gp.epi.bias = p->w + b_off;
   gp.epi.resid = resid; gp.epi.ldr = N;
@@ -69,30 +86,26 @@ int linear_fwd(const void* a_base, bool fp16_ops, bool at0, const oob_layer_para
     gp.epi.act = gelu ? ACT_GELU : ACT_NONE;
     gp.epi.planes = planes_out; gp.epi.ldp = N; gp.epi.plane_stride = (long)M * N; gp.epi.nplanes_out = nplanes_out;
   }
-  if (fp16_ops) return gemm_launch(act_planes_h(a_base, M, K, at0), 0, weight_planes_h(p, w_off, K, N, at0), 1, gp, st);
-  return gemm_launch(act_planes(a_base, M, K), 0, weight_planes(p, w_off, K, N), 1, gp, st);
+  return gemm_launch(f.fwd.act(a_base, M, K), 0, f.fwd.weight(p, w_off, K, N), 1, gp, st);
 }
 // dA[M,K] = dY[M,N] . W[K,N]^T  (optionally * gelu'(aux), planes out)
-// dy.fp16 selects the operand family: fp16 pairs (3 products; weights' pair) or bf16 x 3 (6 products)
-int linear_dgrad(const PlaneMat& dy, const oob_layer_params* p, long w_off, int M, int N, int K, int nsplit, float* dA,
-                 const float* dgelu_aux, bf16* planes_out, int nplanes_out, cudaStream_t st) {
-  GemmParams gp{M, K, N, dy.fp16 ? 2 : nsplit, epi_none()};
+int linear_dgrad(const Formats& f, const PlaneMat& dy, const oob_layer_params* p, long w_off, int M, int N, int K,
+                 float* dA, const float* dgelu_aux, bf16* planes_out, int nplanes_out, cudaStream_t st) {
+  GemmParams gp{M, K, N, f.bwd_nsplit, epi_none()};
   gp.epi.d = dA; gp.epi.ldd = K;
   if (dgelu_aux) { gp.epi.act = ACT_DGELU; gp.epi.aux = dgelu_aux; gp.epi.ldaux = K; }
   if (planes_out) {
     gp.epi.planes = planes_out; gp.epi.ldp = K; gp.epi.plane_stride = (long)M * K; gp.epi.nplanes_out = nplanes_out;
   }
-  return gemm_launch(dy, 0, dy.fp16 ? weight_planes_h(p, w_off, K, N, true) : weight_planes(p, w_off, K, N), 0, gp, st);
+  return gemm_launch(dy, 0, f.bwd.weight(p, w_off, K, N), 0, gp, st);
 }
-// dW[K,N] += A[M,K]^T . dY[M,N]
-// `a_base`: the saved activation's plane buffer; with an fp16-pair dy its fp16 pair (planes 3, 4) is the operand and
-// `unscale` (1 / loss scale) is applied to the product before it is accumulated
-int linear_wgrad(const void* a_base, const PlaneMat& dy, const oob_layer_params* p, long w_off, int M, int N, int K,
-                 int nsplit, float unscale, cudaStream_t st) {
-  GemmParams gp{K, N, M, dy.fp16 ? 2 : nsplit, epi_none()};
+// dW[K,N] += unscale * A[M,K]^T . dY[M,N]    (`a_base`: the saved activation's plane buffer)
+int linear_wgrad(const Formats& f, const void* a_base, const PlaneMat& dy, const oob_layer_params* p, long w_off, int M,
+                 int N, int K, cudaStream_t st) {
+  GemmParams gp{K, N, M, f.bwd_nsplit, epi_none()};
   gp.epi.d = p->g + w_off; gp.epi.ldd = N; gp.epi.accumulate = 1;
-  gp.epi.alpha = unscale;
-  return gemm_launch(dy.fp16 ? act_planes_h(a_base, M, K, true) : act_planes(a_base, M, K), 1, dy, 1, gp, st);
+  gp.epi.alpha = f.unscale;
+  return gemm_launch(f.bwd.act(a_base, M, K), 1, dy, 1, gp, st);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -159,11 +172,8 @@ int oob_block_forward(const oob_dims* d, const oob_layer_params* p, const float*
                       void* stream) {
   if (int rc = check_dims(d)) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int M = d->batch * d->seq, E = d->n_embd, ns = d->nsplit;
-  const bool h = d->fwd_fp16 != 0;
-  const bool at0 = d->bwd_fp16 != 0;   // all-fp16 mode: pair-only buffers, nothing reads bf16 planes any more
-  // plane set of every buffer that feeds a forward GEMM (and a wgrad): pair only / bf16 x 3 + pair / bf16 x 3
-  const int np = at0 ? PLANES_H2 : (h ? 5 : 3);
+  const Formats f = formats(d);
+  const int M = d->batch * d->seq, E = d->n_embd, np = f.act_code;
   const BlockOffsets o(E);
   const long ME = (long)M * E;
   int rc;
@@ -171,18 +181,16 @@ int oob_block_forward(const oob_dims* d, const oob_layer_params* p, const float*
                           c->ln1_rstd, M, E, d->ln_eps, st))) return rc;
   // q|k|v go straight to split planes: attention (forward and the recompute in backward) is their only consumer
   // (fp16 pairs when the backward runs on fp16 pairs too: the attention backward reads q|k|v and dO in ONE format)
-  const int ha = d->bwd_fp16 ? 1 : 0;
-  if ((rc = linear_fwd(c->ln1_planes, h, at0, p, o.attn_w, o.attn_b, M, 3 * E, E, ns, nullptr, nullptr,
-                       (bf16*)c->qkv_planes, ha ? PLANES_H2 : 3, false, st))) return rc;
-  if ((rc = attention_fwd((const bf16*)c->qkv_planes, (long)M * 3 * E, ha, c->att, (bf16*)c->att_planes, ME, np, c->lse,
-                          d->batch, d->seq, d->n_head, 64, st))) return rc;
-  if ((rc = linear_fwd(c->att_planes, h, at0, p, o.proj_w, o.proj_b, M, E, E, ns, c->x2, x, nullptr, 0, false, st)))
-    return rc;
+  if ((rc = linear_fwd(f, c->ln1_planes, p, o.attn_w, o.attn_b, M, 3 * E, E, nullptr, nullptr, (bf16*)c->qkv_planes,
+                       f.qkv_code, false, st))) return rc;
+  if ((rc = attention_fwd((const bf16*)c->qkv_planes, (long)M * 3 * E, f.attn_fp16, c->att, (bf16*)c->att_planes, ME, np,
+                          c->lse, d->batch, d->seq, d->n_head, 64, st))) return rc;
+  if ((rc = linear_fwd(f, c->att_planes, p, o.proj_w, o.proj_b, M, E, E, c->x2, x, nullptr, 0, false, st))) return rc;
   if ((rc = layernorm_fwd(c->x2, p->w + o.ln2_w, p->w + o.ln2_b, nullptr, (bf16*)c->ln2_planes, ME, np, c->ln2_mean,
                           c->ln2_rstd, M, E, d->ln_eps, st))) return rc;
-  if ((rc = linear_fwd(c->ln2_planes, h, at0, p, o.fc_w, o.fc_b, M, 4 * E, E, ns, c->fc, nullptr, (bf16*)c->gelu_planes, np,
-                       true, st))) return rc;
-  if ((rc = linear_fwd(c->gelu_planes, h, at0, p, o.proj2_w, o.proj2_b, M, E, 4 * E, ns, y, c->x2, nullptr, 0, false, st)))
+  if ((rc = linear_fwd(f, c->ln2_planes, p, o.fc_w, o.fc_b, M, 4 * E, E, c->fc, nullptr, (bf16*)c->gelu_planes, np, true,
+                       st))) return rc;
+  if ((rc = linear_fwd(f, c->gelu_planes, p, o.proj2_w, o.proj2_b, M, E, 4 * E, y, c->x2, nullptr, 0, false, st)))
     return rc;
   return 0;
 }
@@ -192,18 +200,12 @@ int oob_block_backward(const oob_dims* d, const oob_layer_params* p, const float
                        void* stream) {
   if (int rc = check_dims(d)) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int M = d->batch * d->seq, E = d->n_embd, ns = d->nsplit;
+  const Formats f = formats(d);
+  const int M = d->batch * d->seq, E = d->n_embd, gp_code = f.grad_code;
+  const float us = f.unscale;
   const BlockOffsets o(E);
   const long ME = (long)M * E;
-  // bwd_fp16: activation gradients (dy, dx and the scratch) are multiplied by loss_scale and their planes are fp16
-  // pairs; `us` brings parameter gradients back to true scale where they are produced
-  const bool hb = d->bwd_fp16 != 0;
-  const float us = hb ? 1.0f / d->loss_scale : 1.0f;
-  const int gp_code = hb ? PLANES_H2 : 3;
-  auto gplanes = [&](const void* base, long rows, long cols) {
-    return hb ? grad_planes_h(base, rows, cols) : act_planes(base, rows, cols);
-  };
-  const PlaneMat dyp = gplanes(dy_planes, M, E);
+  const PlaneMat dyp = f.bwd.act(dy_planes, M, E);
   int rc;
   // weight-gradient work goes to the side stream when the caller provided its scratch (see SideState)
   SideState* ss = s->partials_side ? side_state() : nullptr;
@@ -232,37 +234,37 @@ int oob_block_backward(const oob_dims* d, const oob_layer_params* p, const float
 #define OOB_FORK() do { if (ss && (rc = side_fork(ss, st))) return rc; } while (0)
   // ---- MLP ----
   OOB_FORK();   // dy is ready on main
-  if ((rc = linear_wgrad(c->gelu_planes, dyp, p, o.proj2_w, M, E, 4 * E, ns, us, sw))) return rc;
+  if ((rc = linear_wgrad(f, c->gelu_planes, dyp, p, o.proj2_w, M, E, 4 * E, sw))) return rc;
   if ((rc = colsum_accumulate(dy, E, M, E, p->g + o.proj2_b, wparts, us, sw))) return rc;
   if (ss) { OOB_CUDA_OK(cudaEventRecord(ss->dyread, sw)); ss->dyread_pending = true; ss->any_pending = true; }
   // d(fc pre-activation) = (dy . Wp2^T) * gelu'(fc)
-  if ((rc = linear_dgrad(dyp, p, o.proj2_w, M, E, 4 * E, ns, s->dfc, c->fc, (bf16*)s->dfc_planes, gp_code, st)))
+  if ((rc = linear_dgrad(f, dyp, p, o.proj2_w, M, E, 4 * E, s->dfc, c->fc, (bf16*)s->dfc_planes, gp_code, st)))
     return rc;
-  const PlaneMat dfcp = gplanes(s->dfc_planes, M, 4 * E);
+  const PlaneMat dfcp = f.bwd.act(s->dfc_planes, M, 4 * E);
   OOB_FORK();
-  if ((rc = linear_wgrad(c->ln2_planes, dfcp, p, o.fc_w, M, 4 * E, E, ns, us, sw))) return rc;
+  if ((rc = linear_wgrad(f, c->ln2_planes, dfcp, p, o.fc_w, M, 4 * E, E, sw))) return rc;
   if ((rc = colsum_accumulate(s->dfc, 4 * E, M, 4 * E, p->g + o.fc_b, wparts, us, sw))) return rc;
-  if ((rc = linear_dgrad(dfcp, p, o.fc_w, M, 4 * E, E, ns, s->dln, nullptr, nullptr, 0, st))) return rc;
+  if ((rc = linear_dgrad(f, dfcp, p, o.fc_w, M, 4 * E, E, s->dln, nullptr, nullptr, 0, st))) return rc;
   // dx2 = dy + LN2'(dln)
   if ((rc = layernorm_bwd(s->dln, c->x2, c->ln2_mean, c->ln2_rstd, p->w + o.ln2_w, dy, s->dx2, (bf16*)s->dx2_planes,
                           ME, gp_code, p->g + o.ln2_w, p->g + o.ln2_b, s->partials, M, E, us, st))) return rc;
   // ---- attention ----
-  const PlaneMat dx2p = gplanes(s->dx2_planes, M, E);
+  const PlaneMat dx2p = f.bwd.act(s->dx2_planes, M, E);
   OOB_FORK();
-  if ((rc = linear_wgrad(c->att_planes, dx2p, p, o.proj_w, M, E, E, ns, us, sw))) return rc;
+  if ((rc = linear_wgrad(f, c->att_planes, dx2p, p, o.proj_w, M, E, E, sw))) return rc;
   if ((rc = colsum_accumulate(s->dx2, E, M, E, p->g + o.proj_b, wparts, us, sw))) return rc;
-  if ((rc = linear_dgrad(dx2p, p, o.proj_w, M, E, E, ns, s->datt, nullptr, (bf16*)s->datt_planes, gp_code, st)))
+  if ((rc = linear_dgrad(f, dx2p, p, o.proj_w, M, E, E, s->datt, nullptr, (bf16*)s->datt_planes, gp_code, st)))
     return rc;
-  if ((rc = attention_bwd((const bf16*)c->qkv_planes, (long)M * 3 * E, hb ? 1 : 0, c->att, s->datt,
+  if ((rc = attention_bwd((const bf16*)c->qkv_planes, (long)M * 3 * E, f.attn_fp16, c->att, s->datt,
                           (const bf16*)s->datt_planes, ME,
                           c->lse, s->delta, s->dqkv, (bf16*)s->dqkv_planes, (long)M * 3 * E, gp_code, d->batch, d->seq,
                           d->n_head, 64, st))) return rc;
-  const PlaneMat dqkvp = gplanes(s->dqkv_planes, M, 3 * E);
+  const PlaneMat dqkvp = f.bwd.act(s->dqkv_planes, M, 3 * E);
   OOB_FORK();
-  if ((rc = linear_wgrad(c->ln1_planes, dqkvp, p, o.attn_w, M, 3 * E, E, ns, us, sw))) return rc;
+  if ((rc = linear_wgrad(f, c->ln1_planes, dqkvp, p, o.attn_w, M, 3 * E, E, sw))) return rc;
   if ((rc = colsum_accumulate(s->dqkv, 3 * E, M, 3 * E, p->g + o.attn_b, wparts, us, sw))) return rc;
   if (ss) OOB_CUDA_OK(cudaEventRecord(done_ev, sw));
-  if ((rc = linear_dgrad(dqkvp, p, o.attn_w, M, 3 * E, E, ns, s->dln, nullptr, nullptr, 0, st))) return rc;
+  if ((rc = linear_dgrad(f, dqkvp, p, o.attn_w, M, 3 * E, E, s->dln, nullptr, nullptr, 0, st))) return rc;
   // dx = dx2 + LN1'(dln)
   if ((rc = layernorm_bwd(s->dln, x, c->ln1_mean, c->ln1_rstd, p->w + o.ln1_w, s->dx2, dx, (bf16*)dx_planes, ME,
                           gp_code, p->g + o.ln1_w, p->g + o.ln1_b, s->partials, M, E, us, st))) return rc;
@@ -287,47 +289,39 @@ int oob_head_forward(const oob_dims* d, const oob_layer_params* p, const float* 
   if (int rc = check_dims(d)) return rc;
   OOB_CHECK(d->vocab_padded % 64 == 0 && d->vocab_padded >= d->vocab, "vocab_padded must be a multiple of 64");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int M = d->batch * d->seq, E = d->n_embd, V = d->vocab, Vp = d->vocab_padded, ns = d->nsplit;
+  const Formats f = formats(d);
+  const int M = d->batch * d->seq, E = d->n_embd, V = d->vocab, Vp = d->vocab_padded;
   const long ME = (long)M * E;
   int rc;
   // flat layout: ln_f.weight [E], ln_f.bias [E], lm_head.weight [V,E]
-  const bool h = d->fwd_fp16 != 0;
-  const bool at0 = d->bwd_fp16 != 0;
-  if ((rc = layernorm_fwd(x, p->w, p->w + E, nullptr, (bf16*)c->lnf_planes, ME, at0 ? PLANES_H2 : (h ? 5 : 3), c->mean,
-                          c->rstd, M, E, d->ln_eps, st))) return rc;
-  GemmParams gp{M, V, E, h ? 2 : ns, epi_none()};
+  if ((rc = layernorm_fwd(x, p->w, p->w + E, nullptr, (bf16*)c->lnf_planes, ME, f.act_code, c->mean, c->rstd, M, E,
+                          d->ln_eps, st))) return rc;
+  GemmParams gp{M, V, E, f.fwd_nsplit, epi_none()};
   gp.epi.d = c->logits; gp.epi.ldd = Vp;
-  if (h) rc = gemm_launch(act_planes_h(c->lnf_planes, M, E, at0), 0, weight_planes_h(p, 2 * E, V, E, at0), 0, gp, st);
-  else rc = gemm_launch(act_planes(c->lnf_planes, M, E), 0, weight_planes(p, 2 * E, V, E), 0, gp, st);
-  if (rc) return rc;
+  if ((rc = gemm_launch(f.fwd.act(c->lnf_planes, M, E), 0, f.fwd.weight(p, 2 * E, V, E), 0, gp, st))) return rc;
   return cross_entropy(c->logits, Vp, labels, d->batch, d->seq, V, c->row_loss, c->loss, total_loss,
-                       (bf16*)c->dlogits_planes, Vp, (long)M * Vp, d->bwd_fp16 ? PLANES_H2 : 3,
-                       d->bwd_fp16 ? d->loss_scale : 1.0f, st);
+                       (bf16*)c->dlogits_planes, Vp, (long)M * Vp, f.grad_code, d->bwd_fp16 ? d->loss_scale : 1.0f, st);
 }
 
 int oob_head_backward(const oob_dims* d, const oob_layer_params* p, const float* x, const oob_head_ctx* c,
                       oob_bwd_scratch* s, float* dx, void* dx_planes, void* stream) {
   if (int rc = check_dims(d)) return rc;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int M = d->batch * d->seq, E = d->n_embd, V = d->vocab, Vp = d->vocab_padded, ns = d->nsplit;
+  const Formats f = formats(d);
+  const int M = d->batch * d->seq, E = d->n_embd, V = d->vocab, Vp = d->vocab_padded;
   const long ME = (long)M * E;
-  const bool hb = d->bwd_fp16 != 0;
-  const float us = hb ? 1.0f / d->loss_scale : 1.0f;
-  const PlaneMat dlog{reinterpret_cast<const bf16*>(c->dlogits_planes), M, Vp, Vp, (long)M * Vp, hb ? 2 : 3, hb ? 1 : 0};
+  const PlaneMat dlog = f.bwd.act(c->dlogits_planes, M, Vp);
   int rc;
   // d(ln_f out)[M,E] = dlogits[M,V] . Wlm[V,E]
-  GemmParams g1{M, E, V, hb ? 2 : ns, epi_none()};
+  GemmParams g1{M, E, V, f.bwd_nsplit, epi_none()};
   g1.epi.d = s->dln; g1.epi.ldd = E;
-  if ((rc = gemm_launch(dlog, 0, hb ? weight_planes_h(p, 2 * E, V, E, true) : weight_planes(p, 2 * E, V, E), 1, g1, st)))
-    return rc;
+  if ((rc = gemm_launch(dlog, 0, f.bwd.weight(p, 2 * E, V, E), 1, g1, st))) return rc;
   // dWlm[V,E] += dlogits^T . lnf
-  GemmParams g2{V, E, M, hb ? 2 : ns, epi_none()};
-  g2.epi.d = p->g + 2 * E; g2.epi.ldd = E; g2.epi.accumulate = 1; g2.epi.alpha = us;
-  if ((rc = gemm_launch(dlog, 1, hb ? act_planes_h(c->lnf_planes, M, E, true) : act_planes(c->lnf_planes, M, E), 1, g2,
-                        st)))
-    return rc;
-  return layernorm_bwd(s->dln, x, c->mean, c->rstd, p->w, nullptr, dx, (bf16*)dx_planes, ME, hb ? PLANES_H2 : 3, p->g,
-                       p->g + E, s->partials, M, E, us, st);
+  GemmParams g2{V, E, M, f.bwd_nsplit, epi_none()};
+  g2.epi.d = p->g + 2 * E; g2.epi.ldd = E; g2.epi.accumulate = 1; g2.epi.alpha = f.unscale;
+  if ((rc = gemm_launch(dlog, 1, f.bwd.act(c->lnf_planes, M, E), 1, g2, st))) return rc;
+  return layernorm_bwd(s->dln, x, c->mean, c->rstd, p->w, nullptr, dx, (bf16*)dx_planes, ME, f.grad_code, p->g,
+                       p->g + E, s->partials, M, E, f.unscale, st);
 }
 
 }  // extern "C"

@@ -183,15 +183,13 @@ class Layer:
         self.loss_scale = float(16 * 2 ** int(math.floor(math.log2(tokens))))   # dlogits * loss_scale is O(16)
         # placed here because the plane layout depends on it: all-fp16 mode keeps pair-only buffers
         self.bwd_fp16 = 1 if (self.fwd_fp16 and (DEFAULT_BWD_FP16 if bwd_fp16 is None else bwd_fp16)) else 0
-        # plane-set code handed to the producers (include/oobleck_b200.h) and the number of planes allocated.  The
+        # plane-set codes handed to the producers (include/oobleck_b200.h): ``nplanes`` for the weights and every saved
+        # activation a GEMM reads, ``grad_code`` for activation gradients; ``nplane_count`` planes are allocated.  The
         # embedding layer feeds no GEMM (wte / wpe are gathered in fp32): it carries no planes at all.
-        if layer.kind == "embed":
-            self.nplanes = 0
-        elif not self.fwd_fp16:
-            self.nplanes = 3
-        else:
-            self.nplanes = 22 if self.bwd_fp16 else 5
-        self.nplane_count = 2 if self.nplanes == 22 else self.nplanes
+        act_code = L.PLANES_FP16_PAIR if self.bwd_fp16 else (L.PLANES_BF16X3_FP16_PAIR if self.fwd_fp16 else 3)
+        self.nplanes = 0 if layer.kind == "embed" else act_code
+        self.nplane_count = L.planes_count(self.nplanes)
+        self.grad_code = L.PLANES_FP16_PAIR if self.bwd_fp16 else 3
         self.planes = (torch.empty(self.nplane_count, self.plane_stride, dtype=torch.bfloat16, device=self.device)
                        if self.nplanes else None)
         # AdamW step count of THIS layer's moments: travels with exp_avg / exp_avg_sq through reconfigurations so the
@@ -341,8 +339,7 @@ class Layer:
         self.ctx_tensors, self.ctx, self.out, self.saved_in = [], [], [], [None] * self.num_pipe_buffers
         for _ in range(self.num_pipe_buffers):
             if self.spec.kind == "block":
-                # buffers that feed a forward GEMM: pair only (all-fp16 mode) / bf16 x 3 + pair / bf16 x 3
-                np_ = 2 if self.bwd_fp16 else (5 if self.fwd_fp16 else 3)
+                np_ = self.nplane_count     # buffers that feed a forward GEMM and a wgrad
                 t = {"ln1_planes": torch.empty(np_, M, E, **bf), "ln1_mean": torch.empty(M, **f32),
                      "ln1_rstd": torch.empty(M, **f32), "qkv_planes": torch.empty(3, M, 3 * E, **bf),
                      "att": torch.empty(M, E, **f32), "att_planes": torch.empty(np_, M, E, **bf),
@@ -354,7 +351,7 @@ class Layer:
                 self.out.append(torch.empty(self.mb, self.T, E, **f32).requires_grad_(True))
             elif self.spec.kind == "head":
                 Vp = self.dims.vocab_padded
-                t = {"lnf_planes": torch.empty(2 if self.bwd_fp16 else (5 if self.fwd_fp16 else 3), M, E, **bf),
+                t = {"lnf_planes": torch.empty(self.nplane_count, M, E, **bf),
                      "mean": torch.empty(M, **f32),
                      "rstd": torch.empty(M, **f32), "logits": torch.empty(M, Vp, **f32),
                      "dlogits_planes": torch.empty(3, M, Vp, **bf), "row_loss": torch.empty(M, **f32),
@@ -425,7 +422,7 @@ class Layer:
             if grad.planes is None:  # arrived from the next stage as fp32 only: split it here
                 dy_planes = ws.recv_planes
                 L.call("oob_split_planes", C.c_void_p(grad.grad.data_ptr()), C.c_void_p(dy_planes.data_ptr()),
-                       grad.grad.numel(), dy_planes.stride(0), 22 if self.bwd_fp16 else 3, _stream())
+                       grad.grad.numel(), dy_planes.stride(0), self.grad_code, _stream())
                 grad = HiddenGrad(grad.grad, dy_planes)
             dx, dxp = ws.next_dx()
             if dx.data_ptr() == grad.grad.data_ptr():

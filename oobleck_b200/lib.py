@@ -68,6 +68,15 @@ class LayerProfile(C.Structure):           # oob_layer_profile
 
 ACT_NONE, ACT_GELU, ACT_DGELU = 0, 1, 2
 
+# plane-set codes of the producers' ``nplanes`` arguments besides 1..3 bf16 planes (include/oobleck_b200.h)
+PLANES_BF16X3_FP16_PAIR = 5     # OOB_PLANES_BF16X3_FP16_PAIR: bf16 x 3 followed by the fp16 pair
+PLANES_FP16_PAIR = 22           # OOB_PLANES_FP16_PAIR: the fp16 pair only, at planes 0, 1
+
+
+def planes_count(code: int) -> int:
+    """Number of planes a buffer written with plane-set ``code`` holds."""
+    return 2 if code == PLANES_FP16_PAIR else code
+
 _P, _L, _I, _F = C.c_void_p, C.c_long, C.c_int, C.c_float
 _SIGNATURES = {
     "oob_version": (C.c_int, []),

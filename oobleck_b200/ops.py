@@ -30,17 +30,17 @@ def planes_desc(p: torch.Tensor, rows=None, cols=None, fp16: bool = False) -> L.
     rows = rows if rows is not None else p.shape[1]
     cols = cols if cols is not None else p.shape[2]
     if fp16:
-        assert p.shape[0] == 5
+        assert p.shape[0] == L.planes_count(L.PLANES_BF16X3_FP16_PAIR)
         return L.Planes(p[3:].data_ptr(), rows, cols, p.stride(1), p.stride(0), 2, 1)
     return L.Planes(p.data_ptr(), rows, cols, p.stride(1), p.stride(0), min(p.shape[0], 3), 0)
 
 
 def split(x: torch.Tensor, out: torch.Tensor | None = None, nplanes: int = 3) -> torch.Tensor:
-    """fp32 [rows, cols] -> planes [nplanes, rows, cols]."""
+    """fp32 [rows, cols] -> planes [planes_count(nplanes), rows, cols] (``nplanes``: plane-set code)."""
     x = x.contiguous()
     rows, cols = x.shape
     if out is None:
-        out = new_planes(rows, cols, 2 if nplanes == 22 else nplanes, x.device)   # 22 = fp16 pair only
+        out = new_planes(rows, cols, L.planes_count(nplanes), x.device)
     L.call("oob_split_planes", _ptr(x), _ptr(out), x.numel(), out.stride(0), nplanes, _stream())
     return out
 
@@ -58,7 +58,7 @@ def pair_to_float(p: torch.Tensor) -> torch.Tensor:
     return h[0] + h[1] / 2048.0
 
 
-PLANES_FP16_PAIR = 22   # include/oobleck_b200.h OOB_PLANES_FP16_PAIR
+PLANES_FP16_PAIR = L.PLANES_FP16_PAIR
 
 
 def gemm(a: torch.Tensor, a_mn: bool, b: torch.Tensor, b_mn: bool, M: int, N: int, K: int, *, nsplit=NSPLIT_PARITY,

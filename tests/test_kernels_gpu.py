@@ -40,13 +40,13 @@ def test_split_roundtrip():
 def test_split5_fp16_pair():
     """5-plane buffers: planes 0-2 = bf16 x 3 (24 bits, any range), planes 3-4 = fp16 pair (22 bits, |x| < 65504)."""
     x = torch.randn(1000, 72, device=DEV) * torch.logspace(-3, 3, 72, device=DEV)
-    p = ops.split(x, nplanes=5)
+    p = ops.split(x, nplanes=L.PLANES_BF16X3_FP16_PAIR)
     assert rel_err(ops.planes_to_float(p), x) < 1e-7
     back = ops.planes_to_float(p, fp16=True)
     assert ((back - x).abs() <= x.abs() * 2 ** -21 + 2 ** -35).all()   # 22 bits, absolute floor 2^-36
     # saturation instead of inf, and graceful loss of precision below the fp16 normal range
     y = torch.tensor([[1e6, -1e6, 1e-7, 3e-9, 0.0, 65504.0, 1.0, -2.5]], device=DEV)
-    q = ops.planes_to_float(ops.split(y, nplanes=5), fp16=True)
+    q = ops.planes_to_float(ops.split(y, nplanes=L.PLANES_BF16X3_FP16_PAIR), fp16=True)
     assert torch.isfinite(q).all() and abs(q[0, 0].item() - 65504.0 - 65504.0 / 2048) < 1 and q[0, 4] == 0
     assert abs(q[0, 2].item() - 1e-7) < 2 ** -35 and q[0, 6] == 1.0 and q[0, 7] == -2.5
 
@@ -60,8 +60,8 @@ def test_gemm_fp16_pair(a_mn, b_mn, shape):
     torch.manual_seed(M + N + K)
     A = torch.randn(M, K, device=DEV)
     B = torch.randn(K, N, device=DEV) * 0.02
-    ap = ops.split(A.t().contiguous() if a_mn else A, nplanes=5)
-    bp = ops.split(B if b_mn else B.t().contiguous(), nplanes=5)
+    ap = ops.split(A.t().contiguous() if a_mn else A, nplanes=L.PLANES_BF16X3_FP16_PAIR)
+    bp = ops.split(B if b_mn else B.t().contiguous(), nplanes=L.PLANES_BF16X3_FP16_PAIR)
     ref = A.double() @ B.double()
     d = torch.full((M, N), float("nan"), device=DEV)
     ops.gemm(ap, a_mn, bp, b_mn, M, N, K, nsplit=2, d=d, a_fp16=True, b_fp16=True)
@@ -80,10 +80,10 @@ def test_gemm_epilogue_five_planes():
     M, N, K = 256, 384, 320
     A, W = torch.randn(M, K, device=DEV), torch.randn(K, N, device=DEV) * 0.05
     bias = torch.randn(N, device=DEV)
-    ap, wp = ops.split(A, nplanes=5), ops.split(W, nplanes=5)
+    ap, wp = ops.split(A, nplanes=L.PLANES_BF16X3_FP16_PAIR), ops.split(W, nplanes=L.PLANES_BF16X3_FP16_PAIR)
     pre_ref = A.double() @ W.double() + bias.double()
     d = torch.empty(M, N, device=DEV)
-    gp = ops.new_planes(M, N, 5)
+    gp = ops.new_planes(M, N, L.planes_count(L.PLANES_BF16X3_FP16_PAIR))
     ops.gemm(ap, False, wp, True, M, N, K, nsplit=2, d=d, bias=bias, act=L.ACT_GELU, planes_out=gp, a_fp16=True,
              b_fp16=True)
     assert rel_err(d, pre_ref) < 2e-6

@@ -244,10 +244,10 @@ def test_adamw_layer_step_matches_oracle():
                C.c_void_p(torch.cuda.current_stream().cuda_stream))
         oo.adamw_step_(p, g, m, v, step, lr)
         close(l.flat_param, p, f"param after step {step}", rtol=1e-6)
-    if l.nplanes != 22:
+    if l.nplanes != L.PLANES_FP16_PAIR:
         close(l.planes[:3, :l.numel].float().sum(0), p, "bf16 planes track the parameters", rtol=1e-6)
-    if l.nplanes in (5, 22):     # pair at planes 3, 4 of a 5-plane buffer, at 0, 1 of a pair-only one
-        o = 3 if l.nplanes == 5 else 0
+    if l.nplanes in (L.PLANES_BF16X3_FP16_PAIR, L.PLANES_FP16_PAIR):   # pair at planes 3, 4 / at 0, 1 of a pair-only one
+        o = 3 if l.nplanes == L.PLANES_BF16X3_FP16_PAIR else 0
         h = l.planes[o:o + 2, :l.numel].view(torch.float16).float()
         close(h[0] + h[1] / 2048.0, p, "fp16 pair tracks the parameters", rtol=1e-6)
 
