@@ -460,7 +460,7 @@ int attention_fwd_t(const bf16* qkv, long qkv_ps, float* out, bf16* out_planes, 
   using F = Fmt<NPL>;
   const long M = (long)B * T, E = (long)H * AD;
   const PlaneMat qm{qkv, M, 3 * E, 3 * E, qkv_ps, NPL, F::FP16 ? 1 : 0};
-  const CUtensorMap* tqkv;
+  CUtensorMap tqkv;
   if (int rc = tensor_map_3d(&tqkv, qm, TR, NPL)) return rc;
   const size_t smem = 6 * F::TILE + SMEM_SLACK;
   static bool once = false;
@@ -469,7 +469,7 @@ int attention_fwd_t(const bf16* qkv, long qkv_ps, float* out, bf16* out_planes, 
     once = true;
   }
   dim3 grid(H, B, (T + TR - 1) / TR);
-  attn_fwd_sm90_kernel<NPL><<<grid, THREADS, smem, s>>>(*tqkv, out, reinterpret_cast<uint16_t*>(out_planes),
+  attn_fwd_sm90_kernel<NPL><<<grid, THREADS, smem, s>>>(tqkv, out, reinterpret_cast<uint16_t*>(out_planes),
                                                         plane_stride, nplanes, lse, T, H, 1.0f / sqrtf((float)AD));
   OOB_CUDA_OK(cudaGetLastError());
   count_launch();
@@ -484,7 +484,7 @@ int attention_bwd_t(const bf16* qkv, long qkv_ps, const float* out, const float*
   const long M = (long)B * T, E = (long)H * AD;
   const PlaneMat qm{qkv, M, 3 * E, 3 * E, qkv_ps, NPL, F::FP16 ? 1 : 0};
   const PlaneMat dm{dout_planes, M, E, E, do_ps, NPL, F::FP16 ? 1 : 0};
-  const CUtensorMap *tqkv, *tdo;
+  CUtensorMap tqkv, tdo;
   int rc;
   if ((rc = tensor_map_3d(&tqkv, qm, TR, NPL))) return rc;
   if ((rc = tensor_map_3d(&tdo, dm, TR, NPL))) return rc;
@@ -503,11 +503,11 @@ int attention_bwd_t(const bf16* qkv, long qkv_ps, const float* out, const float*
   dim3 grid(H, B, (T + TR - 1) / TR);
   const float scale = 1.0f / sqrtf((float)AD);
   uint16_t* pl = reinterpret_cast<uint16_t*>(dqkv_planes);
-  attn_bwd_kv_sm90_kernel<NPL><<<grid, THREADS, smem_kv, s>>>(*tqkv, *tdo, lse, delta, dqkv, pl, plane_stride,
+  attn_bwd_kv_sm90_kernel<NPL><<<grid, THREADS, smem_kv, s>>>(tqkv, tdo, lse, delta, dqkv, pl, plane_stride,
                                                               nplanes, T, H, scale);
   OOB_CUDA_OK(cudaGetLastError());
   count_launch();
-  attn_bwd_q_sm90_kernel<NPL><<<grid, THREADS, smem_q, s>>>(*tqkv, *tdo, lse, delta, dqkv, pl, plane_stride,
+  attn_bwd_q_sm90_kernel<NPL><<<grid, THREADS, smem_q, s>>>(tqkv, tdo, lse, delta, dqkv, pl, plane_stride,
                                                             nplanes, T, H, scale);
   OOB_CUDA_OK(cudaGetLastError());
   count_launch();

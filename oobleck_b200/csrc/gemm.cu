@@ -70,7 +70,7 @@ struct MapKeyHash {
 static std::atomic<long> g_map_encodes{0};
 long tensor_map_encodes() { return g_map_encodes.load(); }
 
-int tensor_map_3d(const CUtensorMap** out, const PlaneMat& a, int box_rows, int box_planes) {
+int tensor_map_3d(CUtensorMap* out, const PlaneMat& a, int box_rows, int box_planes) {
   thread_local std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
   const MapKey key{a.base, a.rows, a.cols, a.ld, a.plane_stride, a.nplanes, box_rows, box_planes};
   auto it = cache.find(key);
@@ -81,7 +81,7 @@ int tensor_map_3d(const CUtensorMap** out, const PlaneMat& a, int box_rows, int 
     g_map_encodes.fetch_add(1, std::memory_order_relaxed);
     it = cache.emplace(key, m).first;
   }
-  *out = &it->second;
+  *out = it->second;   // a copy: the next miss may clear the cache
   return 0;
 }
 
@@ -168,27 +168,25 @@ int gemm_launch(const PlaneMat& A, int a_mn, const PlaneMat& B, int b_mn, const 
              (!e.planes || ((reinterpret_cast<uintptr_t>(e.planes) & 7) == 0 && (e.ldp & 3) == 0 &&
                             (e.plane_stride & 3) == 0));
   }
-  const CUtensorMap *pta = nullptr, *ptb = nullptr;
+  CUtensorMap ta, tb;
   int rc;
   // K-major operand: stored [MN][K] -> box {64 k, tile rows, planes}; MN-major: stored [K][MN] -> box {64 mn, 64 k rows}
   if (!a_mn) {
     OOB_CHECK(A.rows >= p.M && A.cols >= p.K, "A (K-major) is %ld x %ld, need %d x %d", A.rows, A.cols, p.M, p.K);
-    rc = tensor_map_3d(&pta, PlaneMat{A.base, (long)p.M, (long)p.K, A.ld, A.plane_stride, A.nplanes}, GEMM_BM, p.nsplit);
+    rc = tensor_map_3d(&ta, PlaneMat{A.base, (long)p.M, (long)p.K, A.ld, A.plane_stride, A.nplanes}, GEMM_BM, p.nsplit);
   } else {
     OOB_CHECK(A.rows >= p.K && A.cols >= p.M, "A (M-major) is %ld x %ld, need %d x %d", A.rows, A.cols, p.K, p.M);
-    rc = tensor_map_3d(&pta, PlaneMat{A.base, (long)p.K, (long)p.M, A.ld, A.plane_stride, A.nplanes}, GEMM_BK, p.nsplit);
+    rc = tensor_map_3d(&ta, PlaneMat{A.base, (long)p.K, (long)p.M, A.ld, A.plane_stride, A.nplanes}, GEMM_BK, p.nsplit);
   }
   if (rc) return rc;
   if (!b_mn) {
     OOB_CHECK(B.rows >= p.N && B.cols >= p.K, "B (K-major) is %ld x %ld, need %d x %d", B.rows, B.cols, p.N, p.K);
-    rc = tensor_map_3d(&ptb, PlaneMat{B.base, (long)p.N, (long)p.K, B.ld, B.plane_stride, B.nplanes}, GEMM_BN, p.nsplit);
+    rc = tensor_map_3d(&tb, PlaneMat{B.base, (long)p.N, (long)p.K, B.ld, B.plane_stride, B.nplanes}, GEMM_BN, p.nsplit);
   } else {
     OOB_CHECK(B.rows >= p.K && B.cols >= p.N, "B (N-major) is %ld x %ld, need %d x %d", B.rows, B.cols, p.K, p.N);
-    rc = tensor_map_3d(&ptb, PlaneMat{B.base, (long)p.K, (long)p.N, B.ld, B.plane_stride, B.nplanes}, GEMM_BK, p.nsplit);
+    rc = tensor_map_3d(&tb, PlaneMat{B.base, (long)p.K, (long)p.N, B.ld, B.plane_stride, B.nplanes}, GEMM_BK, p.nsplit);
   }
   if (rc) return rc;
-  const CUtensorMap& ta = *pta;
-  const CUtensorMap& tb = *ptb;
 #define OOB_DISPATCH_MAJORS(F16)                                                  \
   do {                                                                            \
     if (!a_mn && !b_mn) return launch_t<false, false, F16>(ta, tb, p, stream);    \

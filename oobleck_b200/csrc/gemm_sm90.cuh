@@ -269,9 +269,9 @@ struct PlaneMat {
 int gemm_launch(const PlaneMat& A, int a_mn_major, const PlaneMat& B, int b_mn_major, const GemmParams& p,
                 cudaStream_t stream);
 
-// Cached TMA descriptor over a split matrix [nplanes][rows][ld]: box = {64 columns, box_rows, box_planes},
-// SWIZZLE_128B.  The returned pointer is valid until the next call on this host thread.
-int tensor_map_3d(const CUtensorMap** out, const PlaneMat& a, int box_rows, int box_planes);
+// TMA descriptor over a split matrix [nplanes][rows][ld]: box = {64 columns, box_rows, box_planes}, SWIZZLE_128B.
+// Looked up in a per-thread cache and copied into *out.
+int tensor_map_3d(CUtensorMap* out, const PlaneMat& a, int box_rows, int box_planes);
 long tensor_map_encodes();   // cuTensorMapEncodeTiled calls so far (cache misses)
 
 // CUDA-event instrumentation of GEMM launches (bench.py roofline): see oob_gemm_timing_begin/end

@@ -93,7 +93,8 @@ def test_gemm_epilogue_five_planes():
 
 @pytest.mark.parametrize("a_mn", [False, True])
 @pytest.mark.parametrize("b_mn", [False, True])
-@pytest.mark.parametrize("shape", [(128, 128, 64), (256, 384, 512), (304, 200, 136), (1024, 768, 768), (256, 128, 6400)])
+@pytest.mark.parametrize("shape", [(128, 128, 64), (256, 384, 512), (304, 200, 136), (1024, 768, 768), (256, 128, 6400),
+                                   (136, 8, 576), (8, 136, 448)])
 def test_gemm_majors(a_mn, b_mn, shape):
     M, N, K = shape
     A = torch.randn(M, K, device=DEV)
