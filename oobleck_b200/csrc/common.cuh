@@ -34,10 +34,8 @@ void count_launch(int n = 1);
 // ---------------------------------------------------------------------------------------------
 // Split representation.  An fp32 value x is carried to the tensor cores as up to three bf16 planes
 // p0 + p1 + p2 == x to 24 mantissa bits (p0 = bf16(x), p1 = bf16(x - p0), p2 = bf16(x - p0 - p1)).
-// A GEMM with nsplit planes issues the products whose combined weight is >= 2^-8(nsplit-1):
-//   nsplit 1: p0q0                      (bf16 accuracy,  1 MMA)
-//   nsplit 2: + p0q1 + p1q0             (~2^-16,        3 MMAs)
-//   nsplit 3: + p1q1 + p0q2 + p2q0      (~2^-23, fp32-grade, 6 MMAs)   <- parity mode
+// Which plane products a tensor-core product of two split operands issues: the split-product scheme below
+// (split_products, split_kblock).
 typedef __nv_bfloat16 bf16;
 
 // Second operand format: TWO fp16 planes, x ~= h0 + 2^-11 * h1 with h0 = fp16(x), h1 = fp16((x - h0) * 2^11).
@@ -215,16 +213,54 @@ __device__ __forceinline__ void fence_regs(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 #include "wgmma_sm90.inc"
-template <bool F16, int TA, int TB>
-__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
-  if constexpr (F16) wgmma_m64n128_f16<TA, TB>(d, a, b, scale_d);
-  else wgmma_m64n128_bf16<TA, TB>(d, a, b, scale_d);
-}
-template <bool F16, int TA, int TB>
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, int scale_d) {
-  if constexpr (F16) wgmma_m64n64_f16<TA, TB>(d, a, b, scale_d);
+template <int N, bool F16, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64(float (&d)[N / 2], uint64_t a, uint64_t b, int scale_d) {
+  static_assert(N == 64 || N == 128, "m64n64 or m64n128");
+  if constexpr (N == 128) {
+    if constexpr (F16) wgmma_m64n128_f16<TA, TB>(d, a, b, scale_d);
+    else wgmma_m64n128_bf16<TA, TB>(d, a, b, scale_d);
+  } else if constexpr (F16) wgmma_m64n64_f16<TA, TB>(d, a, b, scale_d);
   else wgmma_m64n64_bf16<TA, TB>(d, a, b, scale_d);
 }
+
+// The split-product scheme.  Operands split into ns planes issue the plane products whose combined weight is
+// >= 2^-8(ns-1); product q multiplies A plane split_pa(q) by B plane split_pb(q):
+//   q        0 1 2 3 4 5
+//   A plane  0 0 1 1 0 2
+//   B plane  0 1 0 1 2 0
+//   ns 1: q < 1 (bf16 accuracy); ns 2: q < 3 (~2^-16 on bf16 planes, fp32-grade on fp16 pairs); ns 3: q < 6 (~2^-23)
+// Product 0 accumulates in "main", the others in "corr", folded as main + split_corr_weight * corr: the second plane
+// of an fp16 pair is pre-scaled by H1_SCALE, bf16 planes are not.
+__host__ __device__ constexpr int split_products(int ns) { return ns == 1 ? 1 : (ns == 2 ? 3 : 6); }
+__host__ __device__ constexpr int split_pa(int q) { constexpr int t[6] = {0, 0, 1, 1, 0, 2}; return t[q]; }
+__host__ __device__ constexpr int split_pb(int q) { constexpr int t[6] = {0, 1, 0, 1, 2, 0}; return t[q]; }
+__host__ __device__ constexpr float split_corr_weight(bool f16) { return f16 ? H1_INV_SCALE : 1.0f; }
+
+// Contraction depth of split_kblock: one SWIZZLE_128B tile row of 16-bit elements.
+constexpr int SPLIT_KBLOCK = 64;
+constexpr int SPLIT_ROW_BYTES = 2 * SPLIT_KBLOCK;
+
+// One SPLIT_KBLOCK-deep k-block of the split products into 64 x N accumulators: the k-steps of product 0 into
+// acc_main, then the corrections, k outer and q inner, into acc_corr.  a / b describe plane 0 of SWIZZLE_128B tiles
+// (make_smem_desc): a plane lies A_PLANE / B_PLANE bytes further, a k-step of 16 is 32 B (K-major) or 16 rows
+// (MN-major).  A fresh accumulator is overwritten by its first wgmma.
+template <int N, int NS, bool F16, int TA, int TB, uint32_t A_PLANE, uint32_t B_PLANE>
+__device__ __forceinline__ void split_kblock(uint64_t a, uint64_t b, float (&acc_main)[N / 2], float (&acc_corr)[N / 2],
+                                             int main_fresh, int corr_fresh) {
+  constexpr uint32_t A_KSTEP = TA ? 16 * SPLIT_ROW_BYTES : 32, B_KSTEP = TB ? 16 * SPLIT_ROW_BYTES : 32;
+#pragma unroll
+  for (int k = 0; k < SPLIT_KBLOCK / 16; ++k)
+    wgmma_m64<N, F16, TA, TB>(acc_main, a + ((k * A_KSTEP) >> 4), b + ((k * B_KSTEP) >> 4),
+                              (k == 0 && main_fresh) ? 0 : 1);
+#pragma unroll
+  for (int k = 0; k < SPLIT_KBLOCK / 16; ++k)
+#pragma unroll
+    for (int q = 1; q < split_products(NS); ++q)
+      wgmma_m64<N, F16, TA, TB>(acc_corr, a + ((split_pa(q) * A_PLANE + k * A_KSTEP) >> 4),
+                                b + ((split_pb(q) * B_PLANE + k * B_KSTEP) >> 4),
+                                (k == 0 && q == 1 && corr_fresh) ? 0 : 1);
+}
+
 // Accumulator fragment of an m64nN wgmma: register i of thread (warp w of the warpgroup, lane l) holds
 // row 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1).
 __device__ __forceinline__ int frag_row(int warp_in_wg, int lane, int i) { return 16 * warp_in_wg + (lane >> 2) + 8 * ((i >> 1) & 1); }

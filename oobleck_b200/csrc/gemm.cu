@@ -138,7 +138,7 @@ static int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPara
   const size_t smem = (size_t)stages * stage + overhead;
   TimedLaunch tl{};
   if (g_timing) { tl.a = get_event(); tl.b = get_event(); tl.flops = 2.0 * p.M * p.N * p.K;
-    tl.executed = tl.flops * (p.nsplit == 1 ? 1 : (p.nsplit == 2 ? 3 : 6)); cudaEventRecord(tl.a, stream); }
+    tl.executed = tl.flops * split_products(p.nsplit); cudaEventRecord(tl.a, stream); }
   kern<<<grid, GEMM_THREADS, smem, stream>>>(ta, tb, p, stages);
   OOB_CUDA_OK(cudaGetLastError());
   if (g_timing) { cudaEventRecord(tl.b, stream); g_timed.push_back(tl); }
@@ -153,11 +153,7 @@ int gemm_launch(const PlaneMat& A, int a_mn, const PlaneMat& B, int b_mn, const 
   // operand formats: bf16 x (1..3) planes, or fp16 x (1..2) planes with the second plane pre-scaled by 2^11.  wgmma
   // takes one element type for both operands, so the two must agree.
   OOB_CHECK(A.fp16 == B.fp16, "mixed fp16 / bf16 operands are not supported");
-  p.corr_scale = 1.0f;
-  if (A.fp16) {
-    OOB_CHECK(p.nsplit <= 2, "fp16 planes come in pairs: nsplit must be 1 or 2");
-    if (p.nsplit == 2) p.corr_scale = 1.0f / 2048.0f;
-  }
+  OOB_CHECK(!A.fp16 || p.nsplit <= 2, "fp16 planes come in pairs: nsplit must be 1 or 2");
   OOB_CHECK(A.nplanes >= p.nsplit && B.nplanes >= p.nsplit, "operands carry fewer planes than nsplit");
   OOB_CHECK(!p.epi.planes || planes_code_valid(p.epi.nplanes_out), "GEMM: unknown plane-set code %d", p.epi.nplanes_out);
   {

@@ -48,7 +48,6 @@ struct GemmParams {
   int M, N, K;
   int nsplit;   // planes used from each operand (1..3)
   GemmEpilogue epi;
-  float corr_scale;     // weight of the correction accumulator (2^-11 for fp16 x 2 planes, else 1); gemm_launch
 };
 
 constexpr int GEMM_BM = 128;
@@ -57,6 +56,7 @@ constexpr int GEMM_BK = 64;          // one 128-B swizzle span of 16-bit element
 constexpr int GEMM_THREADS = 256;    // two warpgroups
 constexpr int GEMM_ROWB = GEMM_BK * 2;
 constexpr int GEMM_STAGE_LD = GEMM_BN + 8;   // fp32 staging row stride: the fragment stores are conflict-free
+static_assert(GEMM_BK == SPLIT_KBLOCK && GEMM_ROWB == SPLIT_ROW_BYTES, "a stage's k-block is one split_kblock");
 
 // Accumulation scheme.  The tensor core's fp32 accumulation is not round-to-nearest: over a long contraction its error
 // grows with the number of MMAs.  To keep fp32-grade results for any K:
@@ -116,33 +116,17 @@ __device__ __forceinline__ void epilogue_quad(const GemmEpilogue& ep, long grow,
 
 // All products of one k-block for this warpgroup's 64 rows.  Shared-memory layout of a stage (what the TMA boxes
 // produce): A K-major [plane][128 rows][128 B], A M-major [atom of 64 rows][plane][64 k-rows][128 B]; B likewise with
-// its N index.  Product q uses A plane PA[q] and B plane PB[q]:
-//   q:      0 1 2 3 4 5
-//   A plane 0 0 1 1 0 2      B plane 0 1 0 1 2 0
+// its N index.
 template <int NS, bool A_MN, bool B_MN, bool F16>
 __device__ __forceinline__ void gemm_issue_kblock(uint32_t sa, uint32_t sb, int wg, float (&acc_main)[64],
                                                   float (&acc_corr)[64], int main_fresh, int corr_fresh) {
   constexpr uint32_t A_PLANE = (A_MN ? GEMM_BK : GEMM_BM) * GEMM_ROWB;
   constexpr uint32_t B_PLANE = (B_MN ? GEMM_BK : GEMM_BN) * GEMM_ROWB;
-  constexpr uint32_t A_KSTEP = A_MN ? 16 * GEMM_ROWB : 32;
-  constexpr uint32_t B_KSTEP = B_MN ? 16 * GEMM_ROWB : 32;
   constexpr uint32_t ATOM = NS * GEMM_BK * GEMM_ROWB;   // distance between MN atoms
-  constexpr int NPROD = NS == 1 ? 1 : (NS == 2 ? 3 : 6);
-  constexpr int PA[6] = {0, 0, 1, 1, 0, 2};
-  constexpr int PB[6] = {0, 1, 0, 1, 2, 0};
   const uint32_t a0 = sa + (A_MN ? wg * ATOM : wg * 64 * GEMM_ROWB);
-  const uint64_t a_base = make_smem_desc(a0, A_MN ? ATOM : 0, 8 * GEMM_ROWB);
-  const uint64_t b_base = make_smem_desc(sb, B_MN ? ATOM : 0, 8 * GEMM_ROWB);
-#pragma unroll
-  for (int k = 0; k < GEMM_BK / 16; ++k)
-    wgmma_n128<F16, A_MN, B_MN>(acc_main, a_base + ((k * A_KSTEP) >> 4), b_base + ((k * B_KSTEP) >> 4),
-                                (k == 0 && main_fresh) ? 0 : 1);
-#pragma unroll
-  for (int k = 0; k < GEMM_BK / 16; ++k)
-#pragma unroll
-    for (int q = 1; q < NPROD; ++q)
-      wgmma_n128<F16, A_MN, B_MN>(acc_corr, a_base + ((PA[q] * A_PLANE + k * A_KSTEP) >> 4),
-                                  b_base + ((PB[q] * B_PLANE + k * B_KSTEP) >> 4), (k == 0 && q == 1 && corr_fresh) ? 0 : 1);
+  split_kblock<GEMM_BN, NS, F16, A_MN, B_MN, A_PLANE, B_PLANE>(make_smem_desc(a0, A_MN ? ATOM : 0, 8 * GEMM_ROWB),
+                                                               make_smem_desc(sb, B_MN ? ATOM : 0, 8 * GEMM_ROWB),
+                                                               acc_main, acc_corr, main_fresh, corr_fresh);
 }
 
 // grid (tiles_m, tiles_n): consecutive CTAs share the same B panel (L2 reuse) and stream different A row blocks.
@@ -227,7 +211,7 @@ gemm_planes_sm90_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_
   }
   if (nsplit > 1) {
 #pragma unroll
-    for (int i = 0; i < 64; ++i) racc[i] = fmaf(acc_corr[i], p.corr_scale, racc[i]);
+    for (int i = 0; i < 64; ++i) racc[i] = fmaf(acc_corr[i], split_corr_weight(F16), racc[i]);
   }
 
   // epilogue: every load has been consumed, the ring is dead -> fp32 staging tile [128][GEMM_STAGE_LD]
