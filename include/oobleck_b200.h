@@ -203,6 +203,18 @@ int oob_head_forward(const oob_dims* d, const oob_layer_params* p, const float* 
                      oob_head_ctx* ctx, float* total_loss, void* stream);
 int oob_head_backward(const oob_dims* d, const oob_layer_params* p, const float* x, const oob_head_ctx* ctx,
                       oob_bwd_scratch* s, float* dx, void* dx_planes, void* stream);
+/* Forward-only head (evaluation): loss = CE(lm_head(ln_f(x)), shift(labels)) with the shift and ignored targets of
+ * oob_cross_entropy, but no logits and no dlogits are ever written.  The LM-head GEMM reduces each row of each
+ * 128-column output tile to (max, sum exp) in `partials` (oob_head_eval_partials_floats(B*T, vocab) floats, 8-B
+ * aligned); a second kernel merges them in a fixed order (deterministic).
+ *   lnf_planes   [planes_count(lnf_nplanes)][M][E] scratch: any plane-set code that holds what a forward GEMM reads
+ *                (fwd_fp16: OOB_PLANES_FP16_PAIR or OOB_PLANES_BF16X3_FP16_PAIR; else nsplit..3 or the latter)
+ *   mean, rstd   [M] scratch;  row_loss [M] per-row loss (0 where no target);  loss [1] this micro-batch's mean
+ *   acc          NULL or double[2]: acc[0] += loss, acc[1] += number of targets counted.  total_loss is not touched. */
+long oob_head_eval_partials_floats(int rows, int vocab);
+int oob_head_eval(const oob_dims* d, const oob_layer_params* p, const float* x, const long long* labels,
+                  void* lnf_planes, int lnf_nplanes, float* mean, float* rstd, float* partials, float* row_loss,
+                  float* loss, double* acc, void* stream);
 /* `stream` waits for every weight-gradient kernel queued on the side stream so far (see oob_bwd_scratch) */
 int oob_side_join(void* stream);
 /* 0 = run everything on the caller's stream even when partials_side is set (profiling: clean per-kernel times) */

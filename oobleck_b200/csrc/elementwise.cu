@@ -417,10 +417,12 @@ cross_entropy_kernel(const float* __restrict__ logits, long ldl, const long long
   }
 }
 
-// loss = sum(row_loss) * scale, deterministic single-CTA reduction
+// loss = sum(row_loss) * scale, deterministic single-CTA reduction.  total += loss; acc[0] += loss, acc[1] += the
+// number of contributing targets (the evaluation accumulator); either may be null.
 __global__ void __launch_bounds__(1024) loss_reduce_kernel(const float* __restrict__ row_loss,
                                                            const long long* __restrict__ labels, int rows, int T, int V,
-                                                           float* __restrict__ loss, float* __restrict__ total) {
+                                                           float* __restrict__ loss, float* __restrict__ total,
+                                                           double* __restrict__ acc) {
   __shared__ float sh[32];
   const float nvalid = count_valid_targets(labels, rows, T, V, sh);
   __syncthreads();
@@ -431,6 +433,7 @@ __global__ void __launch_bounds__(1024) loss_reduce_kernel(const float* __restri
     const float l = s * (1.0f / fmaxf(nvalid, 1.f));
     *loss = l;
     if (total) *total += l;
+    if (acc) { acc[0] += l; acc[1] += nvalid; }
   }
 }
 
@@ -445,7 +448,58 @@ int cross_entropy(const float* logits, long ldl, const long long* labels, int B,
                                             plane_stride, nplanes);
   OOB_CUDA_OK(cudaGetLastError());
   count_launch();
-  loss_reduce_kernel<<<1, 1024, 0, s>>>(row_loss, labels, rows, T, V, loss, total_loss);
+  loss_reduce_kernel<<<1, 1024, 0, s>>>(row_loss, labels, rows, T, V, loss, total_loss, nullptr);
+  OOB_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Loss of an evaluation pass from the LM head's row log-sum-exp partials (gemm_sm90.cuh epilogue_row_lse): per row
+// and 128-column tile (max, sum exp(x - max)), and the target's logit already in row_loss.  Shift, ignored targets
+// and the mean are those of cross_entropy_kernel / loss_reduce_kernel.
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+  if (m2 == -INFINITY) return;            // an empty side (lanes past the last tile)
+  if (m == -INFINITY) { m = m2; s = s2; return; }
+  const float mn = fmaxf(m, m2);
+  s = s * expf(m - mn) + s2 * expf(m2 - mn);
+  m = mn;
+}
+
+// One warp per row: lane l merges tiles l, l + 32, ... in order, then an xor butterfly merges the lanes.  The merge is
+// symmetric in its two sides, so every lane ends with the same bits and the result does not depend on timing.
+__global__ void __launch_bounds__(256)
+head_eval_rows_kernel(const float2* __restrict__ part, int ntiles, const long long* __restrict__ labels, int rows, int T,
+                      int V, float* __restrict__ row_loss) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const long long target = row % T < T - 1 ? labels[row + 1] : -1;
+  if (!(target >= 0 && target < V)) {
+    if (lane == 0) row_loss[row] = 0.f;
+    return;
+  }
+  float m = -INFINITY, s = 0.f;
+  const float2* pr = part + (long)row * ntiles;
+  for (int j = lane; j < ntiles; j += 32) {
+    const float2 q = pr[j];
+    lse_merge(m, s, q.x, q.y);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    lse_merge(m, s, m2, s2);
+  }
+  if (lane == 0) row_loss[row] = (m + logf(s)) - row_loss[row];
+}
+
+int head_eval_finalize(const float* partials, int ntiles, const long long* labels, int B, int T, int V,
+                       float* row_loss, float* loss, double* acc, cudaStream_t s) {
+  const int rows = B * T;
+  head_eval_rows_kernel<<<(rows + 7) / 8, 256, 0, s>>>(reinterpret_cast<const float2*>(partials), ntiles, labels,
+                                                       rows, T, V, row_loss);
+  OOB_CUDA_OK(cudaGetLastError());
+  count_launch();
+  loss_reduce_kernel<<<1, 1024, 0, s>>>(row_loss, labels, rows, T, V, loss, nullptr, acc);
   OOB_CUDA_OK(cudaGetLastError());
   count_launch();
   return 0;

@@ -113,7 +113,7 @@ int gemm_timing_end(double* total_ms, double* total_flops, double* executed_flop
   return 0;
 }
 
-template <bool A_MN, bool B_MN, bool F16>
+template <bool A_MN, bool B_MN, bool F16, bool ROW_LSE = false>
 static int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
   static int max_smem = -1;
   if (max_smem < 0) {
@@ -122,7 +122,7 @@ static int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPara
     OOB_CUDA_OK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   }
   static bool attr_set = false;
-  auto kern = gemm_planes_sm90_kernel<A_MN, B_MN, F16>;
+  auto kern = gemm_planes_sm90_kernel<A_MN, B_MN, F16, ROW_LSE>;
   if (!attr_set) {
     OOB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     attr_set = true;
@@ -156,6 +156,12 @@ int gemm_launch(const PlaneMat& A, int a_mn, const PlaneMat& B, int b_mn, const 
   OOB_CHECK(!A.fp16 || p.nsplit <= 2, "fp16 planes come in pairs: nsplit must be 1 or 2");
   OOB_CHECK(A.nplanes >= p.nsplit && B.nplanes >= p.nsplit, "operands carry fewer planes than nsplit");
   OOB_CHECK(!p.epi.planes || planes_code_valid(p.epi.nplanes_out), "GEMM: unknown plane-set code %d", p.epi.nplanes_out);
+  const bool row_lse = p.epi.lse_part != nullptr;
+  OOB_CHECK(!row_lse || (!a_mn && !b_mn), "GEMM: the row log-sum-exp epilogue takes K-major operands");
+  OOB_CHECK(!row_lse || (!p.epi.d && !p.epi.planes), "GEMM: the row log-sum-exp epilogue writes no other output");
+  OOB_CHECK(!row_lse || (p.epi.labels && p.epi.target_logit && p.epi.seq >= 2 &&
+                         (reinterpret_cast<uintptr_t>(p.epi.lse_part) & 7) == 0),
+            "GEMM: the row log-sum-exp epilogue needs labels, seq >= 2, target_logit and an 8-B aligned lse_part");
   {
     GemmEpilogue& e = p.epi;
     auto ok16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -183,6 +189,8 @@ int gemm_launch(const PlaneMat& A, int a_mn, const PlaneMat& B, int b_mn, const 
     rc = tensor_map_3d(&tb, PlaneMat{B.base, (long)p.K, (long)p.N, B.ld, B.plane_stride, B.nplanes}, GEMM_BK, p.nsplit);
   }
   if (rc) return rc;
+  if (row_lse) return A.fp16 ? launch_t<false, false, true, true>(ta, tb, p, stream)
+                             : launch_t<false, false, false, true>(ta, tb, p, stream);
 #define OOB_DISPATCH_MAJORS(F16)                                                  \
   do {                                                                            \
     if (!a_mn && !b_mn) return launch_t<false, false, F16>(ta, tb, p, stream);    \

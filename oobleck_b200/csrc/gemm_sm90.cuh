@@ -42,6 +42,14 @@ struct GemmEpilogue {
   int nplanes_out;      // plane-set code (common.cuh)
   float alpha;          // value = alpha * acc (before bias etc.)
   int vec4;             // set by gemm_launch: every pointer / stride above allows 16-B (fp32) and 8-B (plane) accesses
+  // Row log-sum-exp mode (non-null lse_part; the LM head of an evaluation pass): no output matrix at all.  Per row and
+  // 128-column tile, (max, sum exp(x - max)) over the columns < N goes to lse_part[row * ldpart + tile]; the logit of
+  // the row's shifted target labels[row + 1] (rows with row % seq < seq - 1 only) goes to target_logit[row].
+  float2* lse_part;
+  long ldpart;
+  const long long* labels;
+  int seq;
+  float* target_logit;
 };
 
 struct GemmParams {
@@ -114,6 +122,39 @@ __device__ __forceinline__ void epilogue_quad(const GemmEpilogue& ep, long grow,
   }
 }
 
+// Row log-sum-exp epilogue of tile column `tile_n` from the fp32 staging tile: one warp per row, lane l holds columns
+// 4l..4l+3.  Columns >= N (the tail of the last tile) contribute nothing; column n0 < N always exists, so the max is
+// finite.  The exp / max reductions are xor-butterflies, so each partial is the same bits on every run.
+__device__ __forceinline__ void epilogue_row_lse(const GemmParams& p, const float* stage, int m0, int tile_n, int warp,
+                                                 int lane) {
+  const GemmEpilogue& ep = p.epi;
+  const int n0 = tile_n * GEMM_BN, c0 = n0 + 4 * lane;
+#pragma unroll 1
+  for (int row = warp; row < GEMM_BM; row += GEMM_THREADS / 32) {
+    const long grow = m0 + row;
+    if (grow >= p.M) break;
+    const float4 v = *reinterpret_cast<const float4*>(stage + row * GEMM_STAGE_LD + 4 * lane);
+    const float x[4] = {v.x, v.y, v.z, v.w};
+    float mx = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (c0 + j < p.N) mx = fmaxf(mx, x[j]);
+    mx = warp_max(mx);
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (c0 + j < p.N) s += expf(x[j] - mx);
+    s = warp_sum(s);
+    if (lane == 0) {
+      ep.lse_part[grow * ep.ldpart + tile_n] = make_float2(mx, s);
+      if ((int)(grow % ep.seq) < ep.seq - 1) {
+        const long long y = ep.labels[grow + 1];
+        if (y >= n0 && y < n0 + GEMM_BN && y < p.N) ep.target_logit[grow] = stage[row * GEMM_STAGE_LD + (int)(y - n0)];
+      }
+    }
+  }
+}
+
 // All products of one k-block for this warpgroup's 64 rows.  Shared-memory layout of a stage (what the TMA boxes
 // produce): A K-major [plane][128 rows][128 B], A M-major [atom of 64 rows][plane][64 k-rows][128 B]; B likewise with
 // its N index.
@@ -130,7 +171,9 @@ __device__ __forceinline__ void gemm_issue_kblock(uint32_t sa, uint32_t sb, int 
 }
 
 // grid (tiles_m, tiles_n): consecutive CTAs share the same B panel (L2 reuse) and stream different A row blocks.
-template <bool A_MN, bool B_MN, bool F16>
+// ROW_LSE selects the row log-sum-exp epilogue (epilogue_row_lse) instead of the fused epilogue; the main loop is the
+// same code in both.
+template <bool A_MN, bool B_MN, bool F16, bool ROW_LSE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_planes_sm90_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                         const __grid_constant__ GemmParams p, const int num_stages) {
@@ -226,13 +269,17 @@ gemm_planes_sm90_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_
     }
   }
   __syncthreads();
-  const int gcol = n0 + 4 * lane;
+  if constexpr (ROW_LSE) {
+    epilogue_row_lse(p, stage, m0, blockIdx.y, warp, lane);
+  } else {
+    const int gcol = n0 + 4 * lane;
 #pragma unroll 1
-  for (int row = warp; row < GEMM_BM; row += GEMM_THREADS / 32) {
-    const long grow = m0 + row;
-    if (grow >= p.M) break;
-    const float4 v = *reinterpret_cast<const float4*>(stage + row * GEMM_STAGE_LD + 4 * lane);
-    epilogue_quad(p.epi, grow, gcol, p.N, v);
+    for (int row = warp; row < GEMM_BM; row += GEMM_THREADS / 32) {
+      const long grow = m0 + row;
+      if (grow >= p.M) break;
+      const float4 v = *reinterpret_cast<const float4*>(stage + row * GEMM_STAGE_LD + 4 * lane);
+      epilogue_quad(p.epi, grow, gcol, p.N, v);
+    }
   }
 }
 
@@ -250,6 +297,7 @@ struct PlaneMat {
 };
 
 // D = A.B with A given as [M,K] (a_mn_major=0) or [K,M] (a_mn_major=1); B as [N,K] (0) or [K,N] (1).
+// p.epi.lse_part set: the row log-sum-exp epilogue (both operands K-major, no other output).
 int gemm_launch(const PlaneMat& A, int a_mn_major, const PlaneMat& B, int b_mn_major, const GemmParams& p,
                 cudaStream_t stream);
 

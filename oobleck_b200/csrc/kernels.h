@@ -28,6 +28,10 @@ int embedding_bwd(const long long* ids, const float* dx, float* dwte, float* dwp
 int cross_entropy(const float* logits, long ldl, const long long* labels, int B, int T, int V, float* row_loss,
                   float* loss, float* total_loss, bf16* dplanes, long ldp, long plane_stride, int nplanes,
                   float grad_scale, cudaStream_t s);
+// the loss of an evaluation pass from the LM head's row log-sum-exp partials [B*T][ntiles] (float2), with each row's
+// target logit in row_loss on entry; loss = micro-batch mean, acc (may be null) [0] += loss, [1] += targets counted
+int head_eval_finalize(const float* partials, int ntiles, const long long* labels, int B, int T, int V,
+                       float* row_loss, float* loss, double* acc, cudaStream_t s);
 
 int adamw_step(float* p, const float* g, float* m, float* v, bf16* planes, long plane_stride, int nplanes, long n,
                float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t s);

@@ -303,6 +303,46 @@ int oob_head_forward(const oob_dims* d, const oob_layer_params* p, const float* 
                        (bf16*)c->dlogits_planes, Vp, (long)M * Vp, f.grad_code, d->bwd_fp16 ? d->loss_scale : 1.0f, st);
 }
 
+long oob_head_eval_partials_floats(int rows, int vocab) {
+  return 2L * rows * ((vocab + GEMM_BN - 1) / GEMM_BN);
+}
+
+int oob_head_eval(const oob_dims* d, const oob_layer_params* p, const float* x, const long long* labels,
+                  void* lnf_planes, int lnf_nplanes, float* mean, float* rstd, float* partials, float* row_loss,
+                  float* loss, double* acc, void* stream) {
+  if (int rc = check_dims(d)) return rc;
+  OOB_CHECK(d->vocab_padded % 64 == 0 && d->vocab_padded >= d->vocab, "vocab_padded must be a multiple of 64");
+  OOB_CHECK(planes_code_valid(lnf_nplanes), "head_eval: unknown plane-set code %d", lnf_nplanes);
+  // ln_f's planes feed the LM-head GEMM only: they need just what a forward GEMM reads -- the fp16 pair (fwd_fp16) or
+  // bf16 planes 0..nsplit-1 -- so the pair-only or a 1..3-plane buffer is enough.  The weights are read as in training.
+  const Formats f = formats(d);
+  PlaneView lnf{0, f.fwd_nsplit, 0};
+  if (d->fwd_fp16) {
+    OOB_CHECK(lnf_nplanes == OOB_PLANES_FP16_PAIR || lnf_nplanes == OOB_PLANES_BF16X3_FP16_PAIR,
+              "head_eval: fwd_fp16 reads the fp16 pair, plane-set code %d has none", lnf_nplanes);
+    lnf = lnf_nplanes == OOB_PLANES_FP16_PAIR ? PlaneView{0, 2, 1} : PlaneView{3, 2, 1};
+  } else {
+    OOB_CHECK(lnf_nplanes == OOB_PLANES_BF16X3_FP16_PAIR || (lnf_nplanes <= 3 && lnf_nplanes >= d->nsplit),
+              "head_eval: plane-set code %d holds fewer than nsplit = %d bf16 planes", lnf_nplanes, d->nsplit);
+  }
+  OOB_CHECK(x && labels && lnf_planes && mean && rstd && partials && row_loss && loss, "head_eval: null argument");
+  OOB_CHECK((reinterpret_cast<uintptr_t>(lnf_planes) & 15) == 0, "head_eval: ln_f planes must be 16 B aligned");
+  OOB_CHECK((reinterpret_cast<uintptr_t>(partials) & 7) == 0, "head_eval: the partial buffer must be 8 B aligned");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int M = d->batch * d->seq, E = d->n_embd, V = d->vocab;
+  const int ntiles = (V + GEMM_BN - 1) / GEMM_BN;
+  int rc;
+  if ((rc = layernorm_fwd(x, p->w, p->w + E, nullptr, (bf16*)lnf_planes, (long)M * E, lnf_nplanes, mean, rstd, M, E,
+                          d->ln_eps, st))) return rc;
+  // logits never leave the GEMM: its epilogue reduces every 128-column tile of a row to (max, sum exp) and picks
+  // the target's logit (into row_loss, which the finalize kernel then overwrites with the row's loss)
+  GemmParams gp{M, V, E, f.fwd_nsplit, epi_none()};
+  gp.epi.lse_part = reinterpret_cast<float2*>(partials); gp.epi.ldpart = ntiles;
+  gp.epi.labels = labels; gp.epi.seq = d->seq; gp.epi.target_logit = row_loss;
+  if ((rc = gemm_launch(lnf.act(lnf_planes, M, E), 0, f.fwd.weight(p, 2 * E, V, E), 0, gp, st))) return rc;
+  return head_eval_finalize(partials, ntiles, labels, d->batch, d->seq, V, row_loss, loss, acc, st);
+}
+
 int oob_head_backward(const oob_dims* d, const oob_layer_params* p, const float* x, const oob_head_ctx* c,
                       oob_bwd_scratch* s, float* dx, void* dx_planes, void* stream) {
   if (int rc = check_dims(d)) return rc;

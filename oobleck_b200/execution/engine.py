@@ -18,6 +18,7 @@ from __future__ import annotations
 
 import copy
 import datetime
+import math
 import os
 import queue
 import socket
@@ -56,6 +57,7 @@ class JobArguments:
     microbatch_size: int = 8
     global_microbatch_size: int = 128
     steps: int = 50
+    eval_microbatch_size: int = 8      # sequences per evaluation micro-batch (HF per_device_eval_batch_size)
 
 
 @dataclass
@@ -718,6 +720,7 @@ class OobleckEngine:
         self._notified = False           # a loss notification has arrived and has not been applied yet
         self._args = args
         self._hf_training_args = TrainingArguments(per_device_train_batch_size=args.job.microbatch_size,
+                                                   per_device_eval_batch_size=args.job.eval_microbatch_size,
                                                    max_steps=args.job.steps)
         self._local_rank = local_rank
         self._num_nodes = num_nodes
@@ -1020,6 +1023,59 @@ class OobleckEngine:
         if not self._reconfiguration.poll() and not self._wait_for_notification():
             raise failure if failure is not None else PipelineAborted("step dropped but no loss was announced")
         return False
+
+    # -- evaluation --------------------------------------------------------------------------------------------------
+    def evaluate(self, num_microbatches: int | None = None) -> dict:
+        """Validation loss of the current parameters: a forward-only pass of every pipeline over the first
+        ``num_microbatches`` micro-batches of ``per_device_eval_batch_size`` sequences of the validation split (default:
+        as many as the split holds), split between the pipelines like training micro-batches
+        (``distribute_microbatches``).  The head computes the loss without writing logits (``oob_head_eval``).
+
+        Returns, identically on every rank, ``loss`` (mean of the per-micro-batch mean losses, as HF's evaluation loop
+        reports it), ``perplexity`` = exp(loss) (HF ``run_clm``), ``tokens`` (targets counted) and ``microbatches``.
+        Training is not affected: parameters, gradients, moments, ``total_loss``, the step count, the LR schedule and
+        the training data position stay as they were.  Every call starts at the beginning of the validation split."""
+        mb = self._hf_training_args.per_device_eval_batch_size
+        pipelines = self._reconfiguration._pipelines
+        plan = [p._template for p in pipelines]
+        # checked on every rank before any transfer: a first stage that ran out of data would leave the stages after
+        # it waiting in a receive
+        available = len(self._dataset.dataset["validation"]) // mb
+        if num_microbatches is None:
+            num_microbatches = available
+        if not 1 <= num_microbatches <= available:
+            raise ValueError(f"evaluate(): {num_microbatches} micro-batches of {mb} sequences asked for, the validation "
+                             f"split holds {available}")
+        counts = self.distribute_microbatches(plan, num_microbatches)
+        my_index = next(i for i, p in enumerate(pipelines) if p is self._pipeline)
+        loader = OobleckDataLoader(self._hf_training_args, self._dataset, LoaderType.Evaluation, my_index, counts, 0, 0,
+                                   shuffle=False, device_resident=self._device_resident)
+        res = self._pipeline.evaluate(self._model, loader, counts[my_index], mb)
+        total = torch.zeros(3, dtype=torch.float64)
+        if res is not None and self._pipeline.execution._shard_id == 0:   # one rank per pipeline reports
+            total[0], total[1], total[2] = res[0], counts[my_index], res[1]
+        group = self._eval_group()
+        if group is not False:
+            device = self._pipeline.device
+            t = total.to(device)
+            dist.all_reduce(t, group=group)
+            total = t.cpu()
+        loss = float(total[0]) / float(total[1])
+        return {"loss": loss, "perplexity": math.exp(loss), "tokens": int(total[2]), "microbatches": int(total[1])}
+
+    def _eval_group(self):
+        """Communicator over every rank of the current pipelines: None = the world, False = this rank alone."""
+        if not dist.is_initialized():
+            return False
+        ranks = sorted(r for p in self._reconfiguration._pipelines for r in p._ranks)
+        if len(ranks) <= 1:
+            return False
+        if not self._reconfigured and len(ranks) == dist.get_world_size():
+            return None
+        key = tuple(ranks)
+        if key not in _COMMUNICATORS:
+            _COMMUNICATORS[key] = _new_member_group(key, self._comm_timeout)
+        return _COMMUNICATORS[key]
 
     def _make_job_group(self):
         """Elastic runs: the communicator of the per-step vote -- every rank that currently trains."""

@@ -103,6 +103,55 @@ class StageWorkspace:
         L.call("oob_side_join", _stream())
 
 
+class EvalWorkspace:
+    """Forward-only temporaries of one stage at the evaluation micro-batch size (``Layer.evaluate``).  Nothing is saved
+    for a backward, so ONE ``oob_block_ctx`` serves every block of the stage, two ping-pong buffers carry the hidden
+    state from layer to layer, and the head needs ln_f's planes and the LM head's row partials, never logits.
+    ``acc`` accumulates (sum of micro-batch mean losses, targets counted) on the device."""
+
+    def __init__(self, microbatch: int, seq: int, n_embd: int, n_head: int, vocab: int, device: torch.device):
+        self.mb, self.T = microbatch, seq
+        M, E = microbatch * seq, n_embd
+        self.device = device
+        f32 = dict(dtype=torch.float32, device=device)
+        self.hidden = [torch.empty(microbatch, seq, E, **f32) for _ in range(2)]
+        self._n_embd, self._n_head, self._vocab = E, n_head, vocab
+        self._ctx: dict[int, tuple] = {}      # plane count -> (tensors, oob_block_ctx)
+        self._head: dict[int, dict] = {}      # ln_f plane count -> tensors
+        self.acc = torch.zeros(2, dtype=torch.float64, device=device)
+
+    def next_hidden(self, avoid: torch.Tensor | None = None) -> torch.Tensor:
+        """A hidden buffer that is not ``avoid`` (the layer's input)."""
+        a = avoid.data_ptr() if avoid is not None else None
+        return self.hidden[1] if self.hidden[0].data_ptr() == a else self.hidden[0]
+
+    def block_ctx(self, nplanes: int) -> OobBlockCtx:
+        if nplanes not in self._ctx:
+            M, E, H = self.mb * self.T, self._n_embd, self._n_head
+            f32 = dict(dtype=torch.float32, device=self.device)
+            bf = dict(dtype=torch.bfloat16, device=self.device)
+            t = {"ln1_planes": torch.empty(nplanes, M, E, **bf), "ln1_mean": torch.empty(M, **f32),
+                 "ln1_rstd": torch.empty(M, **f32), "qkv_planes": torch.empty(3, M, 3 * E, **bf),
+                 "att": torch.empty(M, E, **f32), "att_planes": torch.empty(nplanes, M, E, **bf),
+                 "lse": torch.empty(self.mb * H * self.T, **f32), "x2": torch.empty(M, E, **f32),
+                 "ln2_planes": torch.empty(nplanes, M, E, **bf), "ln2_mean": torch.empty(M, **f32),
+                 "ln2_rstd": torch.empty(M, **f32), "fc": torch.empty(M, 4 * E, **f32),
+                 "gelu_planes": torch.empty(nplanes, M, 4 * E, **bf)}
+            self._ctx[nplanes] = (t, OobBlockCtx(**{k: v.data_ptr() for k, v in t.items()}))
+        return self._ctx[nplanes][1]
+
+    def head_buffers(self, nplanes: int) -> dict:
+        if nplanes not in self._head:
+            M, E = self.mb * self.T, self._n_embd
+            f32 = dict(dtype=torch.float32, device=self.device)
+            self._head[nplanes] = {
+                "lnf_planes": torch.empty(nplanes, M, E, dtype=torch.bfloat16, device=self.device),
+                "mean": torch.empty(M, **f32), "rstd": torch.empty(M, **f32),
+                "partials": torch.empty(L.load().oob_head_eval_partials_floats(M, self._vocab), **f32),
+                "row_loss": torch.empty(M, **f32), "loss": torch.zeros(1, **f32)}
+        return self._head[nplanes]
+
+
 @dataclass
 class HiddenGrad:
     """Gradient w.r.t. a hidden state travelling backwards through a stage: fp32 + (optionally) its planes."""
@@ -141,6 +190,12 @@ class Layer:
     def make_workspace(cls, model, microbatch_size: int, device) -> "StageWorkspace":
         spec = model.layers[0]
         return StageWorkspace(microbatch_size, spec.n_positions, spec.n_embd, spec.n_head, torch.device(device))
+
+    @classmethod
+    def make_eval_workspace(cls, model, microbatch_size: int, device) -> "EvalWorkspace":
+        spec = model.layers[0]
+        return EvalWorkspace(microbatch_size, spec.n_positions, spec.n_embd, spec.n_head, spec.vocab_size,
+                             torch.device(device))
 
     def __init__(self, layer_id: int, layer: StageLayerSpec, process_group=None, pre_stream=None, post_stream=None, *,
                  microbatch_size: int, num_pipe_buffers: int, workspace: StageWorkspace | None = None,
@@ -438,6 +493,45 @@ class Layer:
                C.c_void_p(g.data_ptr()), C.c_void_p(g.data_ptr() + self.spec.vocab_size * E * 4), self.mb, self.T, E,
                (1.0 / self.loss_scale) if self.bwd_fp16 else 1.0, _stream())
         return None
+
+    # -- evaluation ----------------------------------------------------------------------------------------------------
+    def evaluate(self, inputs: tuple, eval_ws: EvalWorkspace) -> tuple:
+        """Forward-only pass of this layer at the evaluation micro-batch size ``eval_ws.mb``: tuple in, tuple out like
+        ``forward``.  Writes only ``eval_ws``: contexts, ``saved_in``, ``out``, gradients, moments and every loss of
+        the training path are untouched.  The head returns ``(loss,)`` and adds into ``eval_ws.acc``."""
+        kind = self.spec.kind
+        if self._state.sharded:
+            self.unshard_params()     # the same all-gather a forward runs (a no-op unless the shards changed)
+        E, B, T = self.spec.n_embd, eval_ws.mb, eval_ws.T
+        if kind == "embed":
+            input_ids, _attention_mask, labels = inputs
+            assert input_ids.dtype == torch.int64 and input_ids.is_contiguous() and input_ids.numel() == B * T
+            y = eval_ws.next_hidden()
+            w = self._state.full_param
+            L.call("oob_embedding_fwd", C.c_void_p(input_ids.data_ptr()), C.c_void_p(w.data_ptr()),
+                   C.c_void_p(w.data_ptr() + self.spec.vocab_size * E * 4), C.c_void_p(y.data_ptr()), B * T, T, E,
+                   _stream())
+            return y, labels
+        hidden, labels = inputs
+        assert hidden.dtype == torch.float32 and hidden.is_contiguous() and hidden.numel() == B * T * E
+        dims = OobDims(B, T, E, self.dims.n_head, self.dims.vocab, self.dims.vocab_padded, self.dims.ln_eps,
+                       self.dims.nsplit, self.fwd_fp16, self.bwd_fp16, self.loss_scale)
+        p = self._params_struct()
+        if kind == "block":
+            y = eval_ws.next_hidden(avoid=hidden)
+            L.call("oob_block_forward", C.byref(dims), C.byref(p), C.c_void_p(hidden.data_ptr()),
+                   C.c_void_p(y.data_ptr()), C.byref(eval_ws.block_ctx(self.nplane_count)), _stream())
+            return y, labels
+        assert labels.dtype == torch.int64 and labels.is_contiguous()
+        # ln_f's planes feed only the LM-head GEMM: the fp16 pair when the forward reads pairs, else nsplit bf16 planes
+        lnf_code = L.PLANES_FP16_PAIR if self.fwd_fp16 else self.nsplit
+        t = eval_ws.head_buffers(L.planes_count(lnf_code))
+        L.call("oob_head_eval", C.byref(dims), C.byref(p), C.c_void_p(hidden.data_ptr()),
+               C.c_void_p(labels.data_ptr()), C.c_void_p(t["lnf_planes"].data_ptr()), lnf_code,
+               C.c_void_p(t["mean"].data_ptr()), C.c_void_p(t["rstd"].data_ptr()),
+               C.c_void_p(t["partials"].data_ptr()), C.c_void_p(t["row_loss"].data_ptr()),
+               C.c_void_p(t["loss"].data_ptr()), C.c_void_p(eval_ws.acc.data_ptr()), _stream())
+        return (t["loss"][0],)
 
     # -- data parallel -----------------------------------------------------------------------------------------------
     def reduce_gradients(self, process_groups: dict, async_op: bool = False):

@@ -94,6 +94,12 @@ class NvlinkRingTransport(DistTransport):
         base = _align(hidden.numel() * hidden.element_size()) if hidden is not None else 0
         return max(computed, base + extra)
 
+    def reserve_link(self, peer_rank: int, like) -> None:
+        """Create the link with ``peer_rank`` now, sized for tuples shaped like ``like`` (may be meta tensors), unless
+        it exists.  An evaluation pass that runs before the first training step sizes the link for the training
+        tuples it sends in slices of, so that they still fit afterwards."""
+        self._link(peer_rank, like)
+
     def send_tuple(self, tensors, dest_rank: int, kind: str):
         tensors = [t.detach().contiguous() for t in tensors]
         link = self._link(dest_rank, tensors)

@@ -30,8 +30,8 @@ import torch
 import torch.distributed as dist
 
 from .dataloader import OobleckDataLoader, OobleckSampler
-from .schedule import (BackwardPass, ForwardPass, LoadMicroBatch, OobleckPipelineSchedule, RecvActivation, RecvGrad,
-                       SendActivation, SendGrad)
+from .schedule import (BackwardPass, ForwardPass, LoadMicroBatch, OobleckEvalSchedule, OobleckPipelineSchedule,
+                       RecvActivation, RecvGrad, SendActivation, SendGrad)
 from .utils import DTYPE_TO_ID, ID_TO_DTYPE, zero_grads
 
 __all__ = ["OobleckPipelineSchedule", "PipelineExecution", "PipelineCommunication", "OobleckPipeline", "RankGroup",
@@ -470,6 +470,91 @@ class OobleckPipeline:
     def reset_iterator(self):
         self.execution._data_iterator = iter(self.execution._dataloader)
 
+    # -- evaluation -----------------------------------------------------------------------------------------------
+    def evaluate(self, model, dataloader, num_microbatches: int, microbatch_size: int) -> tuple[float, float] | None:
+        """Forward-only pass of this rank's stage over the first ``num_microbatches`` micro-batches of ``dataloader``
+        (``OobleckEvalSchedule``).  Layers run ``Layer.evaluate`` into one per-stage evaluation workspace, allocated on
+        first use and kept; nothing of the training state is touched -- contexts, pipe buffers, gradients, moments,
+        ``total_loss``, the training data position, the step count.  Returns (sum of the micro-batch mean losses,
+        targets counted) on the last stage, None elsewhere.  Raises ``PipelineAborted`` when an inter-stage wait gave up
+        (abort word or watchdog) instead of returning a loss computed from data that never arrived.
+
+        Activations cross a stage boundary in slices of at most one TRAINING micro-batch of sequences: an NVLink link's
+        slot is sized by the first tuple that crosses it (p2p.py), and the training tuples must keep fitting whatever
+        an evaluation sent first."""
+        ex = self.execution
+        layers = ex._layers
+        stages = len(self._template.get_stages())
+        schedule = OobleckEvalSchedule(num_microbatches, stages, self.stage_index)
+        key = (microbatch_size, self.device)
+        if getattr(self, "_eval_ws_key", None) != key:
+            self._eval_ws = self._layer_class().make_eval_workspace(model, microbatch_size, self.device)
+            self._eval_ws_key = key
+        ws = self._eval_ws
+        ws.acc.zero_()
+        spec = layers[0].spec
+        shapes = (microbatch_size, spec.n_positions, spec.n_embd)
+        chunk = self._training_args.per_device_train_batch_size
+        transport = self.communication.transport
+        data = iter(dataloader)
+        inputs = outputs = None
+        for cmds in schedule:
+            for cmd in cmds:
+                if isinstance(cmd, LoadMicroBatch):
+                    batch = next(data)
+                    inputs = tuple(t.to(self.device, non_blocking=True) for t in batch.values())
+                elif isinstance(cmd, RecvActivation):
+                    inputs = self._recv_eval_activations(shapes, chunk)
+                elif isinstance(cmd, ForwardPass):
+                    transport.before_compute()    # the previous micro-batch's send may still read the hidden buffer
+                    x = inputs
+                    for layer in layers:
+                        x = layer.evaluate(x, ws)
+                    outputs, inputs = x, None
+                else:
+                    self._send_eval_activations(outputs, shapes, chunk)
+        if self.device.type == "cuda":
+            torch.cuda.synchronize()       # every wait has either seen its data or given up
+        if hasattr(transport, "aborted") and transport.aborted():
+            raise PipelineAborted("evaluation: an inter-stage transfer was abandoned")
+        if not self.is_last_stage():
+            return None
+        acc = ws.acc.cpu()
+        return float(acc[0]), float(acc[1])
+
+    def _layer_class(self):
+        if self._layer_cls is not None:
+            return self._layer_cls
+        from .layer import Layer
+        return Layer
+
+    def _eval_link_template(self, shapes, chunk: int) -> tuple:
+        """Shape of a training activation tuple (what sizes an NVLink link), without memory."""
+        _, T, E = shapes
+        return (torch.empty(chunk, T, E, device="meta"), torch.empty(chunk, T, dtype=torch.int64, device="meta"))
+
+    def _send_eval_activations(self, outputs: tuple, shapes, chunk: int) -> None:
+        transport, peer = self.communication.transport, self.communication.next_rank
+        if hasattr(transport, "reserve_link"):
+            transport.reserve_link(peer, self._eval_link_template(shapes, chunk))
+        hidden, labels = outputs
+        for s in range(0, hidden.shape[0], chunk):
+            transport.send_tuple((hidden[s:s + chunk], labels[s:s + chunk]), peer, "act")
+
+    def _recv_eval_activations(self, shapes, chunk: int) -> tuple:
+        transport, peer = self.communication.transport, self.communication.prev_rank
+        if hasattr(transport, "reserve_link"):
+            transport.reserve_link(peer, self._eval_link_template(shapes, chunk))
+        B, T, E = shapes
+        parts = []
+        for s in range(0, B, chunk):
+            c = min(chunk, B - s)
+            buf = (torch.empty(c, T, E, device=self.device), torch.empty(c, T, dtype=torch.int64, device=self.device))
+            parts.append(transport.recv_activation_tuple(buf, peer))
+        if len(parts) == 1:
+            return tuple(t.contiguous() for t in parts[0])
+        return torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
+
     # -- construction ---------------------------------------------------------------------------------------------
     def _optimizer_factory(self):
         if self._layer_cls is not None and hasattr(self._layer_cls, "optimizer_factory"):
@@ -544,6 +629,7 @@ class OobleckPipeline:
             stages=len(self._template.get_stages()),
             stage_id=my_stage_index,
         )
+        self.stage_index = my_stage_index
         num_pipe_buffers = self.train_schedule.num_pipe_buffers()
 
         layer_cls = self._layer_cls

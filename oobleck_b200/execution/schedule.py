@@ -92,3 +92,37 @@ class OobleckPipelineSchedule:
 
     def __iter__(self):
         return iter(self.program)
+
+
+class OobleckEvalSchedule:
+    """Forward-only program of one stage (``OobleckPipeline.evaluate``): one step per micro-batch,
+
+        RecvActivation (not on the first stage), LoadMicroBatch (first stage), ForwardPass, SendActivation (not last).
+
+    Every stage receives only from its predecessor and sends only to its successor, in micro-batch order, so the stages
+    form a chain that blocking transfers cannot deadlock (tests/test_evaluate_gloo.py simulates it).  Nothing waits for
+    a backward, so one pipe buffer suffices: a micro-batch's activations have left the stage before the next arrives."""
+
+    def __init__(self, micro_batches: int, stages: int, stage_id: int):
+        assert 0 <= stage_id < stages and micro_batches >= 0
+        self.micro_batches = micro_batches
+        self.stages = stages
+        self.stage_id = stage_id
+        first, last = stage_id == 0, stage_id == stages - 1
+        self.program = []
+        for _ in range(micro_batches):
+            cmds: list[PipeInstruction] = []
+            if not first:
+                cmds.append(RecvActivation(0))
+            if first:
+                cmds.append(LoadMicroBatch(0))
+            cmds.append(ForwardPass(0))
+            if not last:
+                cmds.append(SendActivation(0))
+            self.program.append(cmds)
+
+    def num_pipe_buffers(self) -> int:
+        return 1
+
+    def __iter__(self):
+        return iter(self.program)

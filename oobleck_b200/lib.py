@@ -108,6 +108,8 @@ _SIGNATURES = {
     "oob_head_forward": (_I, [C.POINTER(OobDims), C.POINTER(OobLayerParams), _P, _P, C.POINTER(OobHeadCtx), _P, _P]),
     "oob_head_backward": (_I, [C.POINTER(OobDims), C.POINTER(OobLayerParams), _P, C.POINTER(OobHeadCtx),
                                C.POINTER(OobBwdScratch), _P, _P, _P]),
+    "oob_head_eval_partials_floats": (C.c_long, [_I, _I]),
+    "oob_head_eval": (_I, [C.POINTER(OobDims), C.POINTER(OobLayerParams), _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "oob_side_join": (_I, [_P]),
     "oob_side_stream_enable": (_I, [_I]),
     "oob_p2p_header_bytes": (C.c_long, []),
