@@ -137,6 +137,21 @@ def _new_member_group(ranks, timeout=None):
         c10d._hash_ranks_to_str = orig
 
 
+def _communicator(ranks, timeout):
+    """The process-wide communicator of the rank set ``ranks`` (any order), created on first use."""
+    key = tuple(sorted(ranks))
+    if key not in _COMMUNICATORS:
+        _COMMUNICATORS[key] = _new_member_group(key, timeout)
+    return _COMMUNICATORS[key]
+
+
+def _moved_state(layer) -> list[torch.Tensor]:
+    """What moves when a layer changes owner: ``state_tensors()`` and its AdamW step count as a one-element int64
+    tensor on the same device."""
+    return list(layer.state_tensors()) + [torch.tensor([layer.opt_step], dtype=torch.int64,
+                                                       device=layer.flat_param.device)]
+
+
 # ---- data parallel -------------------------------------------------------------------------------------------------
 class DataParallelEngine:
     def __init__(self, engine, pipelines: list[OobleckPipeline], new_group=None):
@@ -161,10 +176,7 @@ class DataParallelEngine:
             # without re-creating the world group (engine.py:539-593 tears the NCCL world down and re-inits it)
             if not dist.is_initialized() or len(ranks) <= 1 or my_rank not in ranks:
                 return None
-            key = tuple(sorted(ranks))
-            if key not in _COMMUNICATORS:
-                _COMMUNICATORS[key] = _new_member_group(key, engine._comm_timeout)
-            return _COMMUNICATORS[key]
+            return _communicator(ranks, engine._comm_timeout)
 
         make = new_group or _make
         cache: dict[tuple[int, ...], Any] = {}
@@ -209,7 +221,7 @@ class DataParallelEngine:
         engine.py:404-412, layer.py:290-291.)  One bucket per layer: the flat gradient is already contiguous."""
         pgs = self._groups_of(layer)
         if pgs is None:
-            if not getattr(layer, "sharded", False):
+            if not layer.sharded:
                 return
             pgs = {}       # no replica, but the stage shards the layer: its reduce-scatter starts now all the same
         import ctypes as C
@@ -277,10 +289,7 @@ class PeerShadow:
         for s in range(P):                                   # same creation order on both members of a pair
             a, b = self.stage_ranks[(s - 1) % P], self.stage_ranks[s]      # holder, owner
             if me in (a, b):
-                key = tuple(sorted((a, b)))
-                if key not in _COMMUNICATORS:
-                    _COMMUNICATORS[key] = _new_member_group(key, engine._comm_timeout)
-                self.groups[(a, b)] = _COMMUNICATORS[key]
+                self.groups[(a, b)] = _communicator((a, b), engine._comm_timeout)
             if me == a:
                 for l in self.stage_layers[s]:
                     n = engine._model.layers[l].num_params
@@ -310,9 +319,7 @@ class PeerShadow:
             if me == b:
                 for layer in mine:
                     if layer.layer_id in self.stage_layers[s]:
-                        step = torch.tensor([int(getattr(layer, "opt_step", 0))], dtype=torch.int64,
-                                            device=layer.flat_param.device)
-                        for t in list(layer.state_tensors()) + [step]:
+                        for t in _moved_state(layer):
                             works.append(dist.broadcast(t, src=b, group=self.groups[(a, b)], async_op=True))
             if me == a:
                 for l in self.stage_layers[s]:
@@ -582,19 +589,16 @@ class ReconfigurationEngine:
                         else:
                             new_layer.load_flat_(old_layer.flat_param)
                 if dp_group.group is not None:
-                    tensors = (new_layer.state_tensors() if hasattr(new_layer, "state_tensors")
-                               else [new_layer.flat_param])
-                    step = torch.tensor([int(getattr(new_layer, "opt_step", 0))], dtype=torch.int64,
-                                        device=new_layer.flat_param.device)
-                    for t in tensors + [step]:
+                    tensors = _moved_state(new_layer)
+                    step = tensors[-1]
+                    for t in tensors:
                         works.append((dist.broadcast(t, src=src, group=dp_group.group, async_op=True), new_layer,
                                       step if t is step else None))
         for work, layer, step in works:
             if work is not None:
                 work.wait()
             if step is not None and layer is not None:
-                if hasattr(layer, "opt_step"):
-                    layer.opt_step = int(step.item())
+                layer.opt_step = int(step.item())
                 layer.refresh_planes()
         # no world barrier (engine.py:308): a lost rank can never join it; the broadcasts above are the only ordering
         if torch.cuda.is_available():
@@ -630,19 +634,15 @@ class ReconfigurationEngine:
                 tensors = shadow.held[layer_index]
             else:
                 old_layer = next(l for l in engine._pipeline.execution._layers if l.layer_id == layer_index)
-                tensors = list(old_layer.state_tensors()) + [torch.tensor(
-                    [int(getattr(old_layer, "opt_step", 0))], dtype=torch.int64, device=old_layer.flat_param.device)]
+                tensors = _moved_state(old_layer)
             if new_layer is not None and my_rank in dsts:      # the source is one of the new owners: local copy
                 for dst_t, src_t in zip(new_layer.state_tensors(), tensors[:3]):
                     dst_t.copy_(src_t)
                 out.append((None, new_layer, tensors[3].clone()))
         else:
-            tensors = list(new_layer.state_tensors()) + [torch.zeros(1, dtype=torch.int64,
-                                                                     device=new_layer.flat_param.device)]
+            tensors = _moved_state(new_layer)     # receive buffers: every value is overwritten by the broadcast
         if len(members) > 1:
-            if members not in _COMMUNICATORS:
-                _COMMUNICATORS[members] = _new_member_group(members, engine._comm_timeout)
-            group = _COMMUNICATORS[members]
+            group = _communicator(members, engine._comm_timeout)
             for i, t in enumerate(tensors):
                 w = dist.broadcast(t, src=src, group=group, async_op=True)
                 is_step = i == len(tensors) - 1
@@ -835,9 +835,7 @@ class OobleckEngine:
         # my stage may be waiting for a neighbour that is lost -- or alive but already dropping the step: release it
         pipeline = getattr(self, "_pipeline", None)
         if pipeline is not None and pipeline.communication is not None:
-            transport = getattr(pipeline.communication, "transport", None)
-            if transport is not None and hasattr(transport, "abort"):
-                transport.abort()
+            pipeline.communication.transport.abort()
         # communicators that contain a lost rank can never complete anything again
         for key in [k for k in _COMMUNICATORS if lost & set(k)]:
             group = _COMMUNICATORS.pop(key)
@@ -854,7 +852,7 @@ class OobleckEngine:
         ex = self._pipeline.execution
         overlap = (self._agent_pipe is None and self._pipeline.device.type == "cuda"
                    and os.environ.get("OOB_DP_OVERLAP", "1") == "1"
-                   and any(self._dp_engine._groups_of(l) is not None or getattr(l, "sharded", False)
+                   and any(self._dp_engine._groups_of(l) is not None or l.sharded
                            for l in ex._layers))
         ex.grad_ready_hook = self._dp_engine.layer_ready if overlap else None
 
@@ -972,8 +970,7 @@ class OobleckEngine:
                 self._pipeline.train()
                 if on_gpu:
                     torch.cuda.synchronize()      # every wait of this step has either seen its data or given up
-                transport = getattr(self._pipeline.communication, "transport", None)
-                if transport is not None and hasattr(transport, "aborted") and transport.aborted():
+                if self._pipeline.communication.transport.aborted():
                     raise PipelineAborted("an inter-stage transfer was abandoned")
             except (PipelineAborted, RuntimeError) as e:
                 ok, failure = False, e
@@ -993,8 +990,7 @@ class OobleckEngine:
             try:
                 self._dp_engine.do_allreduce()
                 for layer in self._pipeline.execution._layers:
-                    if hasattr(layer, "prepare_gradient_for_optim"):
-                        layer.prepare_gradient_for_optim()
+                    layer.prepare_gradient_for_optim()
                 if on_gpu:
                     torch.cuda.synchronize()
                 if self._dp_engine.touches(self._lost_ranks):
@@ -1072,10 +1068,7 @@ class OobleckEngine:
             return False
         if not self._reconfigured and len(ranks) == dist.get_world_size():
             return None
-        key = tuple(ranks)
-        if key not in _COMMUNICATORS:
-            _COMMUNICATORS[key] = _new_member_group(key, self._comm_timeout)
-        return _COMMUNICATORS[key]
+        return _communicator(ranks, self._comm_timeout)
 
     def _make_job_group(self):
         """Elastic runs: the communicator of the per-step vote -- every rank that currently trains."""
@@ -1083,10 +1076,7 @@ class OobleckEngine:
         self._job_group = None
         if self._agent_pipe is None or not dist.is_initialized() or len(self._job_ranks) <= 1:
             return
-        key = tuple(self._job_ranks)
-        if key not in _COMMUNICATORS:
-            _COMMUNICATORS[key] = _new_member_group(key, self._comm_timeout)
-        self._job_group = _COMMUNICATORS[key]
+        self._job_group = _communicator(self._job_ranks, self._comm_timeout)
 
     def _vote(self, ok: bool) -> bool:
         if self._job_group is None:
@@ -1149,7 +1139,4 @@ class OobleckEngine:
             sorted(r for p in self._reconfiguration._pipelines for r in p._ranks)
         if len(alive) <= 1:
             return
-        key = tuple(alive)
-        if key not in _COMMUNICATORS:
-            _COMMUNICATORS[key] = _new_member_group(key, self._comm_timeout)
-        dist.barrier(group=_COMMUNICATORS[key])
+        dist.barrier(group=_communicator(alive, self._comm_timeout))

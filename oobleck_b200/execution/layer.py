@@ -44,6 +44,23 @@ def _round8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
+def alloc_block_ctx(batch: int, seq: int, n_embd: int, n_head: int, nplanes: int,
+                    device: torch.device) -> tuple[dict, OobBlockCtx]:
+    """The activations one block forward saves (``oob_block_ctx``) for ``batch`` sequences: the tensors and the struct
+    of their addresses.  ``nplanes`` planes for every buffer a forward GEMM and a wgrad read."""
+    M, E = batch * seq, n_embd
+    f32 = dict(dtype=torch.float32, device=device)
+    bf = dict(dtype=torch.bfloat16, device=device)
+    t = {"ln1_planes": torch.empty(nplanes, M, E, **bf), "ln1_mean": torch.empty(M, **f32),
+         "ln1_rstd": torch.empty(M, **f32), "qkv_planes": torch.empty(3, M, 3 * E, **bf),
+         "att": torch.empty(M, E, **f32), "att_planes": torch.empty(nplanes, M, E, **bf),
+         "lse": torch.empty(batch * n_head * seq, **f32), "x2": torch.empty(M, E, **f32),
+         "ln2_planes": torch.empty(nplanes, M, E, **bf), "ln2_mean": torch.empty(M, **f32),
+         "ln2_rstd": torch.empty(M, **f32), "fc": torch.empty(M, 4 * E, **f32),
+         "gelu_planes": torch.empty(nplanes, M, 4 * E, **bf)}
+    return t, OobBlockCtx(**{k: v.data_ptr() for k, v in t.items()})
+
+
 def init_tensors(layer, device) -> None:
     """oobleck/execution/layer.py:26-37 (called by planning/profiler.py:272-274 for every ``model.layers`` entry before
     profiling): put the layer's tensors on ``device``.  The reference fills parameters with ``torch.rand`` ("TODO: must
@@ -127,17 +144,7 @@ class EvalWorkspace:
 
     def block_ctx(self, nplanes: int) -> OobBlockCtx:
         if nplanes not in self._ctx:
-            M, E, H = self.mb * self.T, self._n_embd, self._n_head
-            f32 = dict(dtype=torch.float32, device=self.device)
-            bf = dict(dtype=torch.bfloat16, device=self.device)
-            t = {"ln1_planes": torch.empty(nplanes, M, E, **bf), "ln1_mean": torch.empty(M, **f32),
-                 "ln1_rstd": torch.empty(M, **f32), "qkv_planes": torch.empty(3, M, 3 * E, **bf),
-                 "att": torch.empty(M, E, **f32), "att_planes": torch.empty(nplanes, M, E, **bf),
-                 "lse": torch.empty(self.mb * H * self.T, **f32), "x2": torch.empty(M, E, **f32),
-                 "ln2_planes": torch.empty(nplanes, M, E, **bf), "ln2_mean": torch.empty(M, **f32),
-                 "ln2_rstd": torch.empty(M, **f32), "fc": torch.empty(M, 4 * E, **f32),
-                 "gelu_planes": torch.empty(nplanes, M, 4 * E, **bf)}
-            self._ctx[nplanes] = (t, OobBlockCtx(**{k: v.data_ptr() for k, v in t.items()}))
+            self._ctx[nplanes] = alloc_block_ctx(self.mb, self.T, self._n_embd, self._n_head, nplanes, self.device)
         return self._ctx[nplanes][1]
 
     def head_buffers(self, nplanes: int) -> dict:
@@ -184,7 +191,6 @@ class Layer:
 
     device_type = "cuda"
     supports_deferred_init = True     # accepts init_values=False (see __init__)
-    supports_sharding = True          # accepts columns=<shard columns of the rank grid> (sharding.py)
 
     @classmethod
     def make_workspace(cls, model, microbatch_size: int, device) -> "StageWorkspace":
@@ -253,10 +259,14 @@ class Layer:
         if init_values:
             self._split_planes()
 
-        E, V = layer.n_embd, layer.vocab_size
-        self.dims = OobDims(self.mb, self.T, E, layer.n_head, V, (V + 63) // 64 * 64, layer.layer_norm_epsilon, nsplit,
-                            self.fwd_fp16, self.bwd_fp16, self.loss_scale)
+        self.dims = self._dims(self.mb)
         self._alloc_contexts()
+
+    def _dims(self, batch: int) -> OobDims:
+        """``oob_dims`` of this layer for micro-batches of ``batch`` sequences."""
+        s, V = self.spec, self.spec.vocab_size
+        return OobDims(batch, self.T, s.n_embd, s.n_head, V, (V + 63) // 64 * 64, s.layer_norm_epsilon, self.nsplit,
+                       self.fwd_fp16, self.bwd_fp16, self.loss_scale)
 
     # -- parameters ------------------------------------------------------------------------------------------------
     @property
@@ -394,15 +404,8 @@ class Layer:
         self.ctx_tensors, self.ctx, self.out, self.saved_in = [], [], [], [None] * self.num_pipe_buffers
         for _ in range(self.num_pipe_buffers):
             if self.spec.kind == "block":
-                np_ = self.nplane_count     # buffers that feed a forward GEMM and a wgrad
-                t = {"ln1_planes": torch.empty(np_, M, E, **bf), "ln1_mean": torch.empty(M, **f32),
-                     "ln1_rstd": torch.empty(M, **f32), "qkv_planes": torch.empty(3, M, 3 * E, **bf),
-                     "att": torch.empty(M, E, **f32), "att_planes": torch.empty(np_, M, E, **bf),
-                     "lse": torch.empty(self.mb * H * self.T, **f32), "x2": torch.empty(M, E, **f32),
-                     "ln2_planes": torch.empty(np_, M, E, **bf), "ln2_mean": torch.empty(M, **f32),
-                     "ln2_rstd": torch.empty(M, **f32), "fc": torch.empty(M, 4 * E, **f32),
-                     "gelu_planes": torch.empty(np_, M, 4 * E, **bf)}
-                self.ctx.append(OobBlockCtx(**{k: v.data_ptr() for k, v in t.items()}))
+                t, ctx = alloc_block_ctx(self.mb, self.T, E, H, self.nplane_count, self.device)
+                self.ctx.append(ctx)
                 self.out.append(torch.empty(self.mb, self.T, E, **f32).requires_grad_(True))
             elif self.spec.kind == "head":
                 Vp = self.dims.vocab_padded
@@ -425,34 +428,38 @@ class Layer:
 
     def forward(self, inputs: tuple, buffer_id: int = 0, total_loss: torch.Tensor | None = None) -> tuple:
         """tuple in, tuple out, like the fx shards (sharding.py:86-96)."""
-        kind = self.spec.kind
         self.saved_in[buffer_id] = inputs
         if self._state.sharded:
             self.unshard_params()
-        if kind == "embed":
-            input_ids, _attention_mask, labels = inputs
-            assert input_ids.dtype == torch.int64 and input_ids.is_contiguous()
-            y = self.out[buffer_id]
-            E = self.spec.n_embd
-            w = self._state.full_param
-            L.call("oob_embedding_fwd", C.c_void_p(input_ids.data_ptr()), C.c_void_p(w.data_ptr()),
-                   C.c_void_p(w.data_ptr() + self.spec.vocab_size * E * 4), C.c_void_p(y.data_ptr()),
-                   self.mb * self.T, self.T, E, _stream())
-            return y, labels
+        if self.spec.kind != "head":
+            return self._forward_into(inputs, self.dims, self.out[buffer_id], self.ctx[buffer_id])
         hidden, labels = inputs
         assert hidden.dtype == torch.float32 and hidden.is_contiguous()
-        p = self._params_struct()
-        if kind == "block":
-            y = self.out[buffer_id]
-            L.call("oob_block_forward", C.byref(self.dims), C.byref(p), C.c_void_p(hidden.data_ptr()),
-                   C.c_void_p(y.data_ptr()), C.byref(self.ctx[buffer_id]), _stream())
-            return y, labels
         assert labels.dtype == torch.int64 and labels.is_contiguous()
+        p = self._params_struct()
         L.call("oob_head_forward", C.byref(self.dims), C.byref(p), C.c_void_p(hidden.data_ptr()),
                C.c_void_p(labels.data_ptr()), C.byref(self.ctx[buffer_id]),
                C.c_void_p(0 if total_loss is None else total_loss.data_ptr()), _stream())
         loss = self.ctx_tensors[buffer_id]["loss"][0]  # 0-dim view, like HF's scalar loss
         return loss, self.ctx_tensors[buffer_id]["logits"]
+
+    def _forward_into(self, inputs: tuple, dims: OobDims, y: torch.Tensor, ctx: OobBlockCtx | None) -> tuple:
+        """Embedding or block forward of ``dims.batch`` sequences into ``y``; a block saves its activations in
+        ``ctx``.  Shared by training (``forward``) and evaluation (``evaluate``)."""
+        M, E = dims.batch * dims.seq, dims.n_embd
+        if self.spec.kind == "embed":
+            input_ids, _attention_mask, labels = inputs
+            assert input_ids.dtype == torch.int64 and input_ids.is_contiguous() and input_ids.numel() == M
+            w = self._state.full_param
+            L.call("oob_embedding_fwd", C.c_void_p(input_ids.data_ptr()), C.c_void_p(w.data_ptr()),
+                   C.c_void_p(w.data_ptr() + self.spec.vocab_size * E * 4), C.c_void_p(y.data_ptr()), M, dims.seq, E,
+                   _stream())
+            return y, labels
+        hidden, labels = inputs
+        assert hidden.dtype == torch.float32 and hidden.is_contiguous() and hidden.numel() == M * E
+        L.call("oob_block_forward", C.byref(dims), C.byref(self._params_struct()), C.c_void_p(hidden.data_ptr()),
+               C.c_void_p(y.data_ptr()), C.byref(ctx), _stream())
+        return y, labels
 
     def backward(self, buffer_id: int, grad: HiddenGrad | None) -> HiddenGrad | None:
         """Hand-written backward of this layer for the micro-batch held in ``buffer_id`` (layer.py:250-260 runs
@@ -502,27 +509,16 @@ class Layer:
         kind = self.spec.kind
         if self._state.sharded:
             self.unshard_params()     # the same all-gather a forward runs (a no-op unless the shards changed)
-        E, B, T = self.spec.n_embd, eval_ws.mb, eval_ws.T
-        if kind == "embed":
-            input_ids, _attention_mask, labels = inputs
-            assert input_ids.dtype == torch.int64 and input_ids.is_contiguous() and input_ids.numel() == B * T
-            y = eval_ws.next_hidden()
-            w = self._state.full_param
-            L.call("oob_embedding_fwd", C.c_void_p(input_ids.data_ptr()), C.c_void_p(w.data_ptr()),
-                   C.c_void_p(w.data_ptr() + self.spec.vocab_size * E * 4), C.c_void_p(y.data_ptr()), B * T, T, E,
-                   _stream())
-            return y, labels
+        assert eval_ws.T == self.T      # the workspace's buffers are sized for the sequences the kernels write
+        dims = self._dims(eval_ws.mb)
+        if kind != "head":
+            ctx = eval_ws.block_ctx(self.nplane_count) if kind == "block" else None
+            return self._forward_into(inputs, dims, eval_ws.next_hidden(avoid=inputs[0]), ctx)
         hidden, labels = inputs
-        assert hidden.dtype == torch.float32 and hidden.is_contiguous() and hidden.numel() == B * T * E
-        dims = OobDims(B, T, E, self.dims.n_head, self.dims.vocab, self.dims.vocab_padded, self.dims.ln_eps,
-                       self.dims.nsplit, self.fwd_fp16, self.bwd_fp16, self.loss_scale)
-        p = self._params_struct()
-        if kind == "block":
-            y = eval_ws.next_hidden(avoid=hidden)
-            L.call("oob_block_forward", C.byref(dims), C.byref(p), C.c_void_p(hidden.data_ptr()),
-                   C.c_void_p(y.data_ptr()), C.byref(eval_ws.block_ctx(self.nplane_count)), _stream())
-            return y, labels
+        assert hidden.dtype == torch.float32 and hidden.is_contiguous()
+        assert hidden.numel() == dims.batch * dims.seq * dims.n_embd
         assert labels.dtype == torch.int64 and labels.is_contiguous()
+        p = self._params_struct()
         # ln_f's planes feed only the LM-head GEMM: the fp16 pair when the forward reads pairs, else nsplit bf16 planes
         lnf_code = L.PLANES_FP16_PAIR if self.fwd_fp16 else self.nsplit
         t = eval_ws.head_buffers(L.planes_count(lnf_code))

@@ -31,7 +31,7 @@ class FusedAdamW:
         for l in self.layers:
             # the bias correction follows the layer's own moments (torch keeps ``step`` per parameter too): a layer
             # that arrives through a reconfiguration brings its count with it, a fresh optimizer does not reset it
-            l.opt_step = getattr(l, "opt_step", 0) + 1
+            l.opt_step += 1
             # a layer sharded over its stage (sharding.py): the update runs on this rank's shard of parameters,
             # reduce-scattered gradient and moments; the planes are split after the next all-gather, not here
             l.prepare_gradient_for_optim()

@@ -152,13 +152,6 @@ class NvlinkRingTransport(DistTransport):
         if self.last_send_event is not None:
             torch.cuda.current_stream().wait_event(self.last_send_event)
 
-    # meta handshake stays on torch.distributed (once per direction); DistTransport._send/_recv of the base class
-    def send_meta(self, buffer: tuple, receiver_rank: int):
-        DistTransport.send_meta(self, buffer, receiver_rank)
-
-    def recv_meta(self, sender_rank: int) -> tuple:
-        return DistTransport.recv_meta(self, sender_rank)
-
     def abort(self):
         """Listener thread: release every kernel of this rank that waits on a neighbour (a host store per mailbox)."""
         self._abort = True

@@ -20,6 +20,7 @@ What changed underneath:
 """
 from __future__ import annotations
 
+import contextlib
 import os
 import threading
 import weakref
@@ -188,14 +189,15 @@ class PipelineExecution:
             grad = HiddenGrad(grad_tensors[0])
         # the step's LAST micro-batch: a layer's accumulated gradient is final as soon as its backward is enqueued, so
         # the data-parallel engine may start that layer's all-reduce under the backward of the layers before it
-        self._bwd_seen = getattr(self, "_bwd_seen", 0) + 1
+        self._bwd_seen += 1
         hook = self.grad_ready_hook if self._bwd_seen == self.pipeline.train_schedule.micro_batches else None
         for layer in reversed(self._layers):
             grad = layer.backward(buffer_id, grad)
             if hook is not None:
                 hook(layer)
+        # the StageWorkspace the layers were built with (a reused layer keeps its own); the oracle layers have none
         ws = getattr(self._layers[0], "workspace", None)
-        if ws is not None and hasattr(ws, "join"):
+        if ws is not None:
             ws.join()     # weight-gradient kernels run on a side stream; the ctx slot is recycled after this pass
         if self.pipeline.device.type == "cuda":
             # the stage inputs were allocated under the forward stream (received activations, H2D copies) but this
@@ -309,6 +311,10 @@ class DistTransport:
     def before_compute(self) -> None:
         """Called before a forward / backward pass is enqueued; blocking transports have nothing to order."""
 
+    def reserve_link(self, peer_rank: int, like) -> None:
+        """Called before an evaluation transfer with the shape of a training tuple; blocking transports size
+        nothing in advance."""
+
 
 class PipelineCommunication:
     """pipeline.py:247-427; attribute names kept (``sent_activation_meta``, ``activation_recv_buf``,
@@ -380,10 +386,9 @@ class OobleckPipeline:
         self._transport_cls = transport_cls
         self._nsplit = nsplit
         self._stage_group_factory = stage_group_factory    # ranks -> communicator of a multi-GPU stage (tests)
-        if layer_cls is not None and hasattr(layer_cls, "device_type"):
-            self.device = torch.device(layer_cls.device_type)
-        else:
-            self.device = torch.device("cuda")           # pipeline.py:446
+        self.device = torch.device(self._layer_class().device_type)     # "cuda" for Layer, like pipeline.py:446
+        self._fwd_stream: torch.cuda.Stream | None = None   # forward-family stream of FB_OVERLAP, made on first use
+        self.profile: list | None = None   # bench.py: a list collects (name, start, end) CUDA events of every pass
         # whether this rank trains with this pipeline (:451)
         self.my_pipeline = bool(_my_rank() in ranks)
         # layer index -> list of ranks (:453-456)
@@ -406,61 +411,45 @@ class OobleckPipeline:
         # independent (weights change only in optimizer_step): with FB_OVERLAP they are enqueued on two CUDA streams,
         # ordered by three kinds of events only -- forward(b) -> backward(b), backward(b) -> next occupant of pipe
         # buffer b, end of step -> optimizer.  The GPU then fills the short last waves / small kernels of one pass
-        # with CTAs of the other.  Issue order (the reference's 1F1B program) is unchanged.
+        # with CTAs of the other.  Issue order (the reference's 1F1B program) is unchanged.  Without FB_OVERLAP (and on
+        # CPU) every instruction runs on the current stream and no ordering event is recorded.
         single_stage = self.is_first_stage() and self.is_last_stage()
         overlap = (FB_OVERLAP and self.device.type == "cuda" and torch.cuda.is_available()
                    and (single_stage or FB_OVERLAP_PP))
-        prof = getattr(self, "profile", None)   # bench.py: CUDA-event pairs around every forward / backward pass
+        prof = self.profile
         if overlap:
-            if getattr(self, "_fwd_stream", None) is None:
+            if self._fwd_stream is None:
                 self._fwd_stream = torch.cuda.Stream()
             main, fwd = torch.cuda.current_stream(), self._fwd_stream
             fwd.wait_stream(main)                       # previous optimizer step / reconfiguration copies
-            fwd_done: dict[int, torch.cuda.Event] = {}
-            bwd_done: dict[int, torch.cuda.Event] = {}
+        fwd_done: dict[int, torch.cuda.Event] = {}      # both stay empty without overlap
+        bwd_done: dict[int, torch.cuda.Event] = {}
         forward_family = (LoadMicroBatch, RecvActivation, ForwardPass, SendActivation)
         self.execution._bwd_seen = 0
         for step_cmds in self.train_schedule:
             for cmd in step_cmds:
-                if type(cmd) not in instruction_map:
+                kind = type(cmd)
+                if kind not in instruction_map:
                     raise RuntimeError(f"{self.__class__.__name__} does not understand instruction {repr(cmd)}")
-                timed = prof is not None and type(cmd) in (ForwardPass, BackwardPass)
-                if not overlap:
+                b = cmd.kwargs.get("buffer_id")
+                on_fwd = overlap and kind in forward_family
+                with torch.cuda.stream(fwd) if on_fwd else contextlib.nullcontext():
+                    if on_fwd and b in bwd_done:        # the previous occupant of this pipe buffer has been consumed
+                        fwd.wait_event(bwd_done.pop(b))
+                    elif kind in (BackwardPass, RecvGrad) and b in fwd_done:
+                        main.wait_event(fwd_done.pop(b))
+                    timed = prof is not None and kind in (ForwardPass, BackwardPass)
                     if timed:
                         e0 = torch.cuda.Event(enable_timing=True)
                         e0.record()
-                    instruction_map[type(cmd)](**cmd.kwargs)
-                    if timed:
-                        e1 = torch.cuda.Event(enable_timing=True)
+                    instruction_map[kind](**cmd.kwargs)
+                    if kind in (ForwardPass, BackwardPass) and (overlap or timed):
+                        e1 = torch.cuda.Event(enable_timing=timed)
                         e1.record()
-                        prof.append((type(cmd).__name__, e0, e1))
-                    continue
-                b = cmd.kwargs.get("buffer_id")
-                if type(cmd) in forward_family:
-                    with torch.cuda.stream(fwd):
-                        if b in bwd_done:               # the previous occupant of this pipe buffer has been consumed
-                            fwd.wait_event(bwd_done.pop(b))
+                        if overlap:
+                            (fwd_done if kind is ForwardPass else bwd_done)[b] = e1
                         if timed:
-                            e0 = torch.cuda.Event(enable_timing=True)
-                            e0.record(fwd)
-                        instruction_map[type(cmd)](**cmd.kwargs)
-                        if type(cmd) is ForwardPass:
-                            fwd_done[b] = torch.cuda.Event(enable_timing=timed)
-                            fwd_done[b].record(fwd)
-                            if timed:
-                                prof.append(("ForwardPass", e0, fwd_done[b]))
-                else:
-                    if type(cmd) in (BackwardPass, RecvGrad) and b in fwd_done:
-                        main.wait_event(fwd_done.pop(b))
-                    if timed:
-                        e0 = torch.cuda.Event(enable_timing=True)
-                        e0.record(main)
-                    instruction_map[type(cmd)](**cmd.kwargs)
-                    if type(cmd) is BackwardPass:
-                        bwd_done[b] = torch.cuda.Event(enable_timing=timed)
-                        bwd_done[b].record(main)
-                        if timed:
-                            prof.append(("BackwardPass", e0, bwd_done[b]))
+                            prof.append((kind.__name__, e0, e1))
         if overlap:
             main.wait_stream(fwd)                       # losses, activations still in flight -> optimizer / caller
         for name, pipe_buffers in self.pipe_buffers.items():      # :483-485
@@ -515,7 +504,7 @@ class OobleckPipeline:
                     self._send_eval_activations(outputs, shapes, chunk)
         if self.device.type == "cuda":
             torch.cuda.synchronize()       # every wait has either seen its data or given up
-        if hasattr(transport, "aborted") and transport.aborted():
+        if transport.aborted():
             raise PipelineAborted("evaluation: an inter-stage transfer was abandoned")
         if not self.is_last_stage():
             return None
@@ -535,16 +524,14 @@ class OobleckPipeline:
 
     def _send_eval_activations(self, outputs: tuple, shapes, chunk: int) -> None:
         transport, peer = self.communication.transport, self.communication.next_rank
-        if hasattr(transport, "reserve_link"):
-            transport.reserve_link(peer, self._eval_link_template(shapes, chunk))
+        transport.reserve_link(peer, self._eval_link_template(shapes, chunk))
         hidden, labels = outputs
         for s in range(0, hidden.shape[0], chunk):
             transport.send_tuple((hidden[s:s + chunk], labels[s:s + chunk]), peer, "act")
 
     def _recv_eval_activations(self, shapes, chunk: int) -> tuple:
         transport, peer = self.communication.transport, self.communication.prev_rank
-        if hasattr(transport, "reserve_link"):
-            transport.reserve_link(peer, self._eval_link_template(shapes, chunk))
+        transport.reserve_link(peer, self._eval_link_template(shapes, chunk))
         B, T, E = shapes
         parts = []
         for s in range(0, B, chunk):
@@ -588,11 +575,8 @@ class OobleckPipeline:
     def _stage_communicator(self, ranks: list[int]):
         if self._stage_group_factory is not None:
             return self._stage_group_factory(ranks)
-        from .engine import _COMMUNICATORS, _new_member_group
-        key = tuple(sorted(ranks))
-        if key not in _COMMUNICATORS:
-            _COMMUNICATORS[key] = _new_member_group(key, None)
-        return _COMMUNICATORS[key]
+        from .engine import _communicator
+        return _communicator(ranks, None)
 
     def initialize_distributed_pipeline(self):
         """Per shard column wiring (pipeline.py:582-617): who is my previous / next stage."""
@@ -632,9 +616,7 @@ class OobleckPipeline:
         self.stage_index = my_stage_index
         num_pipe_buffers = self.train_schedule.num_pipe_buffers()
 
-        layer_cls = self._layer_cls
-        if layer_cls is None:
-            from .layer import Layer as layer_cls   # noqa: N813  (needs the CUDA extension; fails loudly otherwise)
+        layer_cls = self._layer_class()
         mb = self._training_args.per_device_train_batch_size
         workspace = layer_cls.make_workspace(model, mb, self.device) if hasattr(layer_cls, "make_workspace") else None
 
@@ -650,18 +632,13 @@ class OobleckPipeline:
                 if existing_layer is not None:
                     # a reused layer keeps its weights, moments and step count; if the new schedule is deeper its
                     # activation contexts are grown in place (a rebuilt Layer would restart from init_flat())
-                    try:
-                        layers.append(layer_cls.create_layer_from_layer(existing_layer, pg, num_pipe_buffers))
-                    except TypeError:   # layer classes with the reference's two-argument signature
-                        layers.append(layer_cls.create_layer_from_layer(existing_layer, pg))
+                    layers.append(layer_cls.create_layer_from_layer(existing_layer, pg, num_pipe_buffers))
                     continue
             extra = {}
             if existing_pipeline is not None and getattr(layer_cls, "supports_deferred_init", False):
                 extra["init_values"] = False      # a layer that appears during a reconfiguration receives its state
             columns = len(self.rank_grid[layer_id])
             if columns > 1:
-                if not getattr(layer_cls, "supports_sharding", False):
-                    raise NotImplementedError(f"{layer_cls.__name__} cannot hold {columns} shard columns")
                 extra["columns"] = columns
             layers.append(layer_cls(layer_id, model.layers[layer_id], pg, None, None, microbatch_size=mb,
                                     num_pipe_buffers=num_pipe_buffers, workspace=workspace, nsplit=self._nsplit,

@@ -56,8 +56,6 @@ class OracleLayer:
     fast_init = False      # bench.py's CPU arm: constant weights (timing does not depend on the values; drawing 1.5 G
                            # normal deviates on the host costs more than the sample itself)
 
-    supports_sharding = True   # same intra-stage sharding as the CUDA layer (oobleck_b200/execution/sharding.py)
-
     # Re-read the torch module's weights from ``flat_param`` before the first forward of every step.  For callers that write ``flat_param``
     # behind the layer's back and never say so -- the reference's own ``_copy_model_states`` broadcasts straight into it
     # (engine.py:284-306), which works there because FSDP's module parameters are views of the flat parameter.  Off by
